@@ -1,6 +1,6 @@
-# Build libnvcomp.so (B200 / sm_100a only) and the CPU oracle.
+# Build libnvcomp.so (H100 / sm_90a only) and the CPU oracle.
 NVCC      ?= /usr/local/cuda/bin/nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall,-Wno-unused-function -Iinclude -Invcomp_b200/csrc
 SRC_DIR   := nvcomp_b200/csrc
 BUILD_DIR := build
@@ -30,14 +30,14 @@ $(BUILD_DIR)/%.o: $(SRC_DIR)/%.cu $(HDRS)
 
 $(LIB): $(OBJS)
 	@mkdir -p nvcomp_b200/lib
-	$(NVCC) $(ARCH) -shared -o $@ $(OBJS) -cudart static
+	$(NVCC) $(ARCH) -shared -Xlinker -soname=libnvcomp.so -o $@ $(OBJS) -cudart static
 
 $(ORACLE_LIB): $(ORACLE_SRCS) $(wildcard oracle/*.h)
 	gcc -O3 -march=x86-64-v2 -fPIC -shared -Wall -o $@ $(ORACLE_SRCS) -ldl -lpthread
 
 build/tests/hlif_test: tests/cpp/hlif_test.cu $(LIB) $(HDRS)
 	@mkdir -p build/tests
-	$(NVCC) $(ARCH) -std=c++17 -O2 -Iinclude $< -o $@ -Lnvcomp_b200/lib -lnvcomp -Xlinker -rpath=$(CURDIR)/nvcomp_b200/lib
+	$(NVCC) $(ARCH) -std=c++17 -O2 -Iinclude $< -o $@ -Lnvcomp_b200/lib -lnvcomp -Xlinker '-rpath=$$ORIGIN/../../nvcomp_b200/lib'
 
 clean:
 	rm -rf $(BUILD_DIR) $(LIB) $(ORACLE_LIB)

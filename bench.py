@@ -21,6 +21,11 @@ Prints ONE JSON line (rank 0):
   cfg1           (--codec lz4) BASELINE configs[0]: 16 x 64 KB LZ4 round trip, latency in us next to liblz4 on one core
   cpu_baseline   liblz4's LZ4_decompress_safe (LZ4) / the oracle port on this box's host cores, median and best
   cfg5           (N > 1, or --cfg5) BASELINE configs[4]: LZ4, 80,000 x 64 KB chunks in total, strong scaling
+
+--dump-outputs DIR writes what the last timed step returned to its caller (rank 0), as .npy files of at most 40 MB in
+all: a fixed, seeded sample of the decompressed chunks (float32, one value per byte), the per-chunk actual sizes and
+statuses, and the per-chunk byte sums of every chunk (float64).  The inputs are seeded, so two builds run with the
+same arguments can be compared file by file.
 """
 from __future__ import annotations
 
@@ -41,6 +46,7 @@ sys.path.insert(0, ROOT)
 CHUNK = 65536
 CHUNKS_PER_GPU = 10000
 CFG5_TOTAL_CHUNKS = 80000
+DUMP_SAMPLE_CHUNKS = 128         # 128 x 64 KB as float32 = 32 MiB, the bulk of a --dump-outputs directory
 FMT = {"lz4": "LZ4", "snappy": "Snappy", "cascaded": "Cascaded", "bitcomp": "Bitcomp", "ans": "ANS"}
 ORACLE_ID = {"lz4": 0, "snappy": 1, "cascaded": 2, "bitcomp": 3, "ans": 4, "liblz4": 5}
 DEFAULT_DATASET = {"lz4": "lz4_mixed", "snappy": "tabular_f32", "cascaded": "sorted_i64",
@@ -62,7 +68,7 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def codec_opts(kind: str, dataset: str):
@@ -602,6 +608,7 @@ def run_gpu(args):
     sampler = ClockSampler(torch.cuda.current_device()) if rank == 0 else None
     m = measure(kind, dataset, n, rank, world, args, sampler)
     w = m["w"]
+    dumped = dump_outputs(w, args.dump_outputs) if args.dump_outputs and rank == 0 else None
     if rank == 0:
         # the timed region lasts only tens of ms; keep the identical load running (untimed) until the
         # sampler has seen ~0.6 s of it, so the clock record describes this kernel under load
@@ -645,7 +652,7 @@ def run_gpu(args):
         "config": {"workload": WORKLOAD_NAME[kind], "codec": kind, "dataset": dataset, "chunks_per_gpu": n,
                    "chunk_bytes": CHUNK, "compression_ratio": round(world * total / m["comp_total_all"], 3),
                    "l2_policy": "inputs larger than L2 (compressed + decompressed footprint per step = "
-                                f"{(total + w.comp_total) / 1e6:.0f} MB vs 126 MB L2)",
+                                f"{(total + w.comp_total) / 1e6:.0f} MB vs 50 MB L2)",
                    "sharding": ("contiguous chunk range per rank; rank 0 owns the compressed slab of every range and scatters "
                                 f"it over NCCL in {DistributedJob.NSLICES} slices per rank, overlapped with the decode of the "
                                 "slices that have arrived (inside `value`)") if world > 1 else "single GPU",
@@ -665,6 +672,8 @@ def run_gpu(args):
                      "kernel": KERNEL_NAME[kind], "avg_launch_ms": round(avg_launch_ms, 4)},
         "clocks": clocks,
     }
+    if dumped is not None:
+        line["dump_outputs"] = dumped
     if world > 1:
         line["distribute"] = {
             "what": "the job's NCCL scatter alone (no decode), warm, max over ranks: bytes leaving rank 0 per step / time",
@@ -710,6 +719,28 @@ def run_gpu(args):
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(w: Workload, out_dir: str) -> dict:
+    """Write what the last decode launch returned to its caller: statuses, actual sizes, the byte sum of every
+    decompressed chunk (float64), and the bytes of a fixed, seeded sample of chunks (float32, one value per byte)."""
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    idx = np.sort(np.random.default_rng(0).choice(w.n, size=min(w.n, DUMP_SAMPLE_CHUNKS), replace=False))
+    chunks = w.out.slab[: w.total].view(w.n, CHUNK)
+    sums = torch.cat([chunks[a: a + 256].to(torch.int32).sum(1) for a in range(0, w.n, 256)])
+    arrays = {
+        "statuses": w.status.cpu().numpy().astype(np.float64),
+        "actual_bytes": w.actual.cpu().numpy().astype(np.float64),
+        "chunk_byte_sums": sums.cpu().numpy().astype(np.float64),
+        "sample_chunk_indices": idx.astype(np.float64),
+        "sample_chunks": chunks[torch.from_numpy(idx).to(chunks.device)].cpu().numpy().astype(np.float32),
+    }
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+    return {"dir": out_dir, "files": sorted(f"{k}.npy" for k in arrays),
+            "bytes": int(sum(a.nbytes for a in arrays.values()))}
 
 
 def run_e2e(w: Workload, args, world, copy_back=True):
@@ -831,7 +862,7 @@ def oracle_compress_batch(lib, kind, dataset, data: np.ndarray):
 
 def run_reference(args):
     """--impl reference: the reference's own implementation of this path is the closed libnvcomp.so
-    (not in /root/reference, not installable: no source, no wheel).  Per the task's tier rules this arm
+    (not in the nvCOMP source tree, not installable: no source, no wheel).  This arm
     times the CPU implementation of the path instead, on all host cores, on the same workload: for LZ4 the decoder
     the reference itself links for its known-answer tests (liblz4's LZ4_decompress_safe, dlopen'd), for the other
     codecs the oracle port (oracle/*.c).  Nothing of libnvcomp.so is loaded on this arm: the synthetic chunks are
@@ -885,7 +916,11 @@ def main():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip per_dataset / foreign_streams (kernel iteration)")
     ap.add_argument("--cfg5", action="store_true", help="also run BASELINE configs[4] (80,000 LZ4 chunks) at N = 1")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed step to DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.impl == "reference":
         run_reference(args)
     else:

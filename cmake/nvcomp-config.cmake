@@ -1,5 +1,5 @@
 # nvcomp-config.cmake -- lets the reference's build system find this library:
-#   cmake -S /root/reference -B build/ref_cmake -Dnvcomp_DIR=/root/repo/cmake -DBUILD_BENCHMARKS=ON
+#   cmake -S <nvCOMP tree> -B oracle/_ref/cmake -Dnvcomp_DIR=<this repo>/cmake -DBUILD_BENCHMARKS=ON
 # satisfies `find_package(nvcomp 3.0.3 REQUIRED)` (reference CMakeLists.txt:18) and provides the imported target
 # `nvcomp::nvcomp` the benchmarks/examples link (reference benchmarks/CMakeLists.txt:28;
 # reference cmake/nvcomp-config.cmake.in:26,38).

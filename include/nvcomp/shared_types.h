@@ -1,6 +1,6 @@
 /*
  * nvcomp/shared_types.h -- status and element-type enums shared by every
- * batched codec of the B200-native nvCOMP-compatible library.
+ * batched codec of the H100-native nvCOMP-compatible library.
  *
  * Boundary evidence (the reference ships no headers; values are pinned by its
  * call sites): nvcompSuccess / nvcompErrorBadChecksum

@@ -1,6 +1,6 @@
-"""nvcomp_b200 -- B200-native batched lossless codecs behind nvCOMP's C API.
+"""nvcomp_b200 -- H100-native batched lossless codecs behind nvCOMP's C API.
 
-The product is ``nvcomp_b200/lib/libnvcomp.so`` (hand-written sm_100a CUDA behind
+The product is ``nvcomp_b200/lib/libnvcomp.so`` (hand-written sm_90a CUDA behind
 the ``nvcompBatched*`` C ABI declared in ``include/nvcomp/*.h``).  This Python
 package is the host-side mirror used by the tests and ``bench.py``: it loads the
 shared library with ctypes and passes raw device pointers; torch is only used

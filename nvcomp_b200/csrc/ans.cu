@@ -1,4 +1,4 @@
-// ans.cu -- batched byte-wise rANS entropy codec for B200 (sm_100a) + its C ABI.
+// ans.cu -- batched byte-wise rANS entropy codec for H100 (sm_90a) + its C ABI.
 //
 // Replaces the closed nvcompBatchedANS* entry points (include/nvcomp/ans.h; reference
 // benchmarks/benchmark_ans_chunked.cu:68-72).  The reference bitstream is undocumented,
@@ -427,7 +427,7 @@ inline size_t ans_scratch_per_cta(size_t max_chunk) {
   const size_t nseg = (max_chunk + kAnsSeg - 1) / kAnsSeg;
   return (nseg ? nseg : 1) * ans_scratch_per_seg();
 }
-constexpr int kAnsMaxCompCtas = kNumSMsB200 * 8;
+constexpr int kAnsMaxCompCtas = 132 * 8;   // workspace cap: 8 CTAs on each of an H100 SXM's 132 SMs
 
 }  // namespace b200
 

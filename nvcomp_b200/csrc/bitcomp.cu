@@ -1,4 +1,4 @@
-// bitcomp.cu -- batched Bitcomp-style typed bit-packing codec for B200 (sm_100a) + C ABI.
+// bitcomp.cu -- batched Bitcomp-style typed bit-packing codec for H100 (sm_90a) + C ABI.
 //
 // Replaces the closed nvcompBatchedBitcomp* entry points (include/nvcomp/bitcomp.h;
 // reference benchmarks/benchmark_bitcomp_chunked.cu:114-118).  Bitcomp is proprietary

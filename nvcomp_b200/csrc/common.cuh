@@ -1,6 +1,6 @@
-// common.cuh -- shared device/host helpers for the B200-native batched codecs.
+// common.cuh -- shared device/host helpers for the H100-native batched codecs.
 //
-// Everything here is internal to libnvcomp.so (sm_100a only).  The public
+// Everything here is internal to libnvcomp.so (sm_90a only).  The public
 // boundary is include/nvcomp/*.h.
 #pragma once
 
@@ -17,7 +17,6 @@ namespace b200 {
 
 constexpr int kWarp = 32;
 constexpr unsigned kFull = 0xffffffffu;
-constexpr int kNumSMsB200 = 148;
 
 // Bytes at the head of every decompress/compress workspace reserved for the
 // persistent chunk scheduler (one 64-bit ticket counter per launch, padded).
@@ -27,8 +26,8 @@ __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 
 // ---------------------------------------------------------------------------
 // Persistent chunk scheduler: every warp (or CTA) pulls the next chunk index
-// from a global ticket counter, so thousands of unequal chunks keep all 148
-// SMs busy until the batch drains (no static wave quantisation).
+// from a global ticket counter, so thousands of unequal chunks keep every
+// SM busy until the batch drains (no static wave quantisation).
 // ---------------------------------------------------------------------------
 struct WarpTicket {
   unsigned long long* counter;  // nullptr -> static grid-stride assignment
@@ -241,10 +240,16 @@ __device__ __forceinline__ void lz_expand_period_from_window(uint8_t* dst, uint3
   }
 }
 
-// Host-side launch helper: number of CTAs for a persistent kernel.
+// SM count of the current device, queried once per device (log.cu); 0 when the query fails.
+int sm_count_for_current_device();
+
+// Host-side launch helper: number of CTAs for a persistent kernel (ctas_per_sm on every SM of the current device,
+// fewer when there is less work).  Correctness does not depend on it: the kernels pull chunks from a ticket or a
+// grid stride, whatever the grid.
 inline int persistent_grid(int ctas_per_sm, size_t work_items, int work_per_cta) {
   size_t need = (work_items + (size_t)work_per_cta - 1) / (size_t)work_per_cta;
-  size_t cap = (size_t)kNumSMsB200 * (size_t)ctas_per_sm;
+  const int sms = sm_count_for_current_device();
+  size_t cap = (size_t)(sms > 0 ? sms : 1) * (size_t)ctas_per_sm;
   size_t g = need < cap ? need : cap;
   return (int)(g == 0 ? 1 : g);
 }

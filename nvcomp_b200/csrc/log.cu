@@ -55,6 +55,16 @@ void log_call(const char* fn, size_t batch, size_t max_chunk, const void* stream
 
 namespace b200 {
 
+int sm_count_for_current_device() {
+  static std::atomic<int> counts[64];   // zero until the device is first seen
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 0;
+  int n = counts[dev].load(std::memory_order_relaxed);
+  if (n == 0 && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess)
+    counts[dev].store(n, std::memory_order_relaxed);
+  return n;
+}
+
 // one non-blocking side stream per device, created on first use and kept for the process (see StreamFork)
 cudaError_t side_stream_for_current_device(cudaStream_t* side) {
   static std::mutex mu;

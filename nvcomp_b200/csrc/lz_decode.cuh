@@ -1,4 +1,4 @@
-// lz_decode.cuh -- block-parallel LZ77 (LZ4 / Snappy) chunk decoder for B200.
+// lz_decode.cuh -- block-parallel LZ77 (LZ4 / Snappy) chunk decoder for H100.
 //
 // One warp owns one chunk.  On tabular data a 64 KB chunk holds 10-15 thousand *short* tokens
 // (4-8 output bytes each), so throughput is bounded by warp-instructions per token, not bytes.

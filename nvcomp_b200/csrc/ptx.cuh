@@ -1,4 +1,4 @@
-// ptx.cuh -- every inline-PTX primitive of the library lives here (sm_100a): explicit shared-space
+// ptx.cuh -- every inline-PTX primitive of the library lives here (sm_90a): explicit shared-space
 // loads / stores on 32-bit shared-window addresses, streaming global vector accesses, mbarrier and
 // TMA bulk-copy wrappers.  The codec headers contain no asm, so tests/emu can re-run their warp-level
 // logic on the host by shadowing this one file (test infrastructure only; the product is CUDA).

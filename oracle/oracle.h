@@ -3,7 +3,7 @@
  *
  * Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl
  * reference leg may load this library; nothing under nvcomp_b200/ links, imports
- * or calls it.  The product path is libnvcomp.so (CUDA, sm_100a) and has no CPU
+ * or calls it.  The product path is libnvcomp.so (CUDA, sm_90a) and has no CPU
  * fallback.
  *
  * What it restates: the reference's codec arithmetic lives in the closed,

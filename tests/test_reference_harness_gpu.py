@@ -1,6 +1,6 @@
 """-m gpu: the reference's OWN benchmarks and examples, compiled unchanged against include/ + libnvcomp.so
-by tools/build_reference_harness.sh (binaries in build/ref/, built where /root/reference exists), run as the
-acceptance harness: every one of them self-verifies (status, sizes, bytes) and prints the reference's
+by oracle/build_reference_harness.sh (binaries in oracle/_ref/, built by build() where the nvCOMP tree exists), run as
+the acceptance harness: every one of them self-verifies (status, sizes, bytes) and prints the reference's
 4-line report (benchmarks/benchmark_template_chunked.cuh:553-617)."""
 import os
 import subprocess
@@ -11,13 +11,13 @@ import pytest
 from conftest import ROOT
 
 pytestmark = pytest.mark.gpu
-BIN = os.path.join(ROOT, "build", "ref")
+BIN = os.path.join(ROOT, "oracle", "_ref", "bin")
 
 
 def _run(name, *args, timeout=600):
     exe = os.path.join(BIN, name)
     if not os.path.exists(exe):
-        pytest.skip(f"{name} not built (tools/build_reference_harness.sh needs /root/reference)")
+        pytest.skip(f"{name} not built (oracle/build_reference_harness.sh needs the nvCOMP source tree)")
     r = subprocess.run([exe, *args], capture_output=True, text=True, timeout=timeout)
     assert r.returncode == 0, (name, r.stdout[-2000:], r.stderr[-2000:])
     return r.stdout
@@ -96,12 +96,12 @@ def test_unsupported_formats_report_not_supported(data_files):
 
 def test_cmake_built_reference_binary_runs():
     """A binary produced by the reference's OWN CMake build against cmake/nvcomp-config.cmake
-    (build/ref_cmake, built where /root/reference exists; PTX-JIT from compute_90 on B200)."""
-    exe = os.path.join(ROOT, "build", "ref_cmake", "bin", "low_level_quickstart_example")
+    (oracle/_ref/cmake, built by oracle/build_reference_harness.sh for sm_90a)."""
+    exe = os.path.join(ROOT, "oracle", "_ref", "cmake", "bin", "low_level_quickstart_example")
     if not os.path.exists(exe):
-        pytest.skip("build/ref_cmake not present")
+        pytest.skip("oracle/_ref/cmake not present")
     r = subprocess.run([exe], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, (r.stdout[-2000:], r.stderr[-2000:])
-    exe = os.path.join(ROOT, "build", "ref_cmake", "bin", "benchmark_snappy_synth")
+    exe = os.path.join(ROOT, "oracle", "_ref", "cmake", "bin", "benchmark_snappy_synth")
     r = subprocess.run([exe, "-b", "200", "-w", "1", "-i", "2"], capture_output=True, text=True, timeout=600)
     assert r.returncode == 0 and "decompression throughput (GB/s)" in r.stdout, (r.stdout[-2000:], r.stderr[-2000:])

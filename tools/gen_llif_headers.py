@@ -85,7 +85,7 @@ TEMPLATE = '''/*
  *
  * Generated by tools/gen_llif_headers.py.  Every entry point replaces the
  * closed libnvcomp.so 3.0.3 symbol of the same name; citations are to the
- * reference tree (/root/reference) call sites that pin the signature.
+ * reference tree's call sites that pin the signature.
  *
  * {note}
  *

@@ -93,7 +93,7 @@ def main():
                               "decomp_GBps": round(total / d_ms / 1e6, 1),
                               "decomp_best_GBps": round(total / d_best / 1e6, 1),
                               "decomp_ms": round(d_ms, 3),
-                              "roofline_frac": round(alg / d_ms / 1e6 / 6587.7, 4), "ok": ok}), flush=True)
+                              "roofline_frac": round(alg / d_ms / 1e6 / 3350.0, 4), "ok": ok}), flush=True)
 
 
 if __name__ == "__main__":
