@@ -12,6 +12,7 @@
 //   u32 magic 'CSC1' | u8 type | u8 num_RLEs | u8 num_deltas | u8 use_bp
 //   u32 uncompressed_bytes, u32 part_bytes, u32 num_parts
 //   u32 part_off[num_parts+1]      byte offsets of each partition payload (8-aligned)
+//   zero pad to 8 bytes (4 bytes when num_parts is odd)
 //   partition payloads
 //   if uncompressed_bytes is not a multiple of the element size: one 8-byte word at part_off[num_parts]
 //   with the trailing uncompressed_bytes % size bytes verbatim (partitions cover the whole elements)
@@ -788,7 +789,7 @@ __device__ uint32_t casc_encode_part(const uint8_t* __restrict__ in, uint32_t n,
   uint32_t off = 8u * (uint32_t)D + ((4u * (uint32_t)D + 7u) & ~7u);
   uint64_t* firsts = (uint64_t*)dst;
   uint32_t* cin = (uint32_t*)(dst + 8u * (uint32_t)D);
-  if (lane < 2 * D) cin[lane] = 0;   // also clears the pad word
+  if (lane < ((D + 1) & ~1)) cin[lane] = 0;   // also clears the pad word (odd D)
   __syncwarp();
   const int L = R > D ? R : D;
   bool had_delta = false;
@@ -864,6 +865,8 @@ cascaded_compress_kernel(const void* const* __restrict__ in_ptrs, const size_t* 
     }
     uint32_t* part_off = (uint32_t*)(out + 20);
     uint32_t off = (20u + 4u * (num_parts + 1) + 7u) & ~7u;
+    // pad bytes are zero: an odd partition count leaves one word between the offset table and the first partition
+    if (lane == 0 && (num_parts & 1u)) part_off[num_parts + 1] = 0u;
     for (uint32_t p = 0; p < num_parts; ++p) {
       if (lane == 0) part_off[p] = off;
       const uint32_t begin = p * P;

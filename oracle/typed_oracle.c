@@ -206,6 +206,8 @@ long oracle_cascaded_compress(const uint8_t* src, size_t n, uint8_t* dst, size_t
   wr32(dst, CSC_MAGIC);
   wr32(dst + 4, (type & 0xff) | ((uint32_t)R << 8) | ((uint32_t)D << 16) | ((uint32_t)(use_bp ? 1 : 0) << 24));
   wr32(dst + 8, (uint32_t)n); wr32(dst + 12, (uint32_t)P); wr32(dst + 16, (uint32_t)np);
+  /* pad bytes are zero: an odd partition count leaves 4 between the offset table and the first partition */
+  memset(dst + 20 + 4 * (np + 1), 0, off - (20 + 4 * (np + 1)));
   size_t cap_e = P / ts;
   uint64_t* cur = (uint64_t*)malloc(8 * (cap_e + 1));
   uint64_t* nxt = (uint64_t*)malloc(8 * (cap_e + 1));
