@@ -46,6 +46,14 @@ constexpr int kLzDecWarps = LZ_DEC_WARPS;
 #define LZ_DEC_CTAS 5
 #endif
 constexpr int kLzDecCtasPerSm = LZ_DEC_CTAS;
+// dense persistent grid, CTAs per SM (see snappy.cu).  5 x 128 threads x 96 registers (61 440 of 65 536) leave no room
+// for a light CTA (128 x 48 = 6 144 registers) until a dense CTA retires; at 4 (49 152) two fit from the start, but the
+// 2 112 dense warps no longer take the 2 500 dense chunks of the LZ4 workload in one wave, and the call gets 30 % slower
+// (DESIGN §3.1).
+#ifndef LZ_DEC_GRID_CTAS
+#define LZ_DEC_GRID_CTAS LZ_DEC_CTAS
+#endif
+constexpr int kLzDecGridCtasPerSm = LZ_DEC_GRID_CTAS;
 // light kernel: no shared memory, 10 CTAs x 4 warps per SM (long copies want many warps in flight)
 #ifndef LZ_LIGHT_CTAS
 #define LZ_LIGHT_CTAS 10
@@ -64,7 +72,9 @@ lz4_decompress_light_kernel(const void* const* __restrict__ comp_ptrs,
   const size_t warp_global = (size_t)blockIdx.x * kLzDecWarps + (threadIdx.x >> 5);
   const size_t warps_total = (size_t)gridDim.x * kLzDecWarps;
   LzWork sched(lists, true, comp_bytes, out_caps, batch, warp_global, warps_total);
+  B200_LZ_TRACE_BEGIN(true);
   for (size_t c = sched.next(lane); c < batch; c = sched.next(lane)) {
+    B200_LZ_TRACE_CHUNK_BEGIN();
     const size_t in_n64 = comp_bytes[c];
     const uint64_t cap = (uint64_t)out_caps[c];
     const uint8_t* in = (const uint8_t*)comp_ptrs[c];
@@ -77,8 +87,10 @@ lz4_decompress_light_kernel(const void* const* __restrict__ comp_ptrs,
       if (actual_bytes) actual_bytes[c] = ok ? (size_t)produced : 0;
       if (statuses) statuses[c] = ok ? nvcompSuccess : nvcompErrorCannotDecompress;
     }
+    B200_LZ_TRACE_CHUNK_END(c, lane);
     __syncwarp();
   }
+  B200_LZ_TRACE_EXIT(warp_global, lane);
 }
 
 __global__ void __launch_bounds__(kLzDecWarps * 32, kLzDecCtasPerSm)
@@ -97,7 +109,9 @@ lz4_decompress_v2_kernel(const void* const* __restrict__ comp_ptrs,
   lz_warp_init(smem_addr(s_ring[w]), lane);
   uint32_t tma_parity = 0;
   LzWork sched(lists, false, comp_bytes, out_caps, batch, warp_global, warps_total);
+  B200_LZ_TRACE_BEGIN(false);
   for (size_t c = sched.next(lane); c < batch; c = sched.next(lane)) {
+    B200_LZ_TRACE_CHUNK_BEGIN();
     const size_t in_n64 = comp_bytes[c];
     const uint64_t cap = (uint64_t)out_caps[c];
     const uint8_t* in = (const uint8_t*)comp_ptrs[c];
@@ -110,8 +124,10 @@ lz4_decompress_v2_kernel(const void* const* __restrict__ comp_ptrs,
       if (actual_bytes) actual_bytes[c] = ok ? (size_t)produced : 0;
       if (statuses) statuses[c] = ok ? nvcompSuccess : nvcompErrorCannotDecompress;
     }
+    B200_LZ_TRACE_CHUNK_END(c, lane);
     __syncwarp();
   }
+  B200_LZ_TRACE_EXIT(warp_global, lane);
 }
 
 // ---------------------------------------------------------------------------
@@ -270,14 +286,14 @@ nvcompStatus_t nvcompBatchedLZ4DecompressAsync(
   if (!comp_ptrs || !comp_bytes || !out_caps || !out_ptrs) return nvcompErrorInvalidValue;
   const LzLists lists = lz_lists_in(temp, temp_bytes, batch);
   if (lists.ctr) {
-    B200_CUDA_TRY(cudaMemsetAsync(lists.ctr, 0, 4 * sizeof(unsigned long long), stream));
+    B200_CUDA_TRY(cudaMemsetAsync(lists.ctr, 0, kLzCounterBytes, stream));
     lz_classify_kernel<<<(unsigned)((batch + 255) / 256), 256, 0, stream>>>(comp_bytes, out_caps, batch, lists);
   }
   // dense kernel on the caller's stream, light kernel beside it (see StreamFork): both are ordered after the ticket
   // reset above and before anything the caller enqueues next
   StreamFork fork;
   B200_CUDA_TRY(fork.begin(stream));
-  const int grid = persistent_grid(kLzDecCtasPerSm, batch, kLzDecWarps);
+  const int grid = persistent_grid(kLzDecGridCtasPerSm, batch, kLzDecWarps);
   lz4_decompress_v2_kernel<<<grid, kLzDecWarps * 32, 0, stream>>>(
       comp_ptrs, comp_bytes, out_caps, actual_bytes, batch, out_ptrs, statuses, lists);
   // both kernels ask for the same shared-memory carveout: an SM does not have to drain and reconfigure between a dense
@@ -294,3 +310,5 @@ nvcompStatus_t nvcompBatchedLZ4DecompressAsync(
 }
 
 }  // extern "C"
+
+B200_LZ_TRACE_EXPORT(lz4)

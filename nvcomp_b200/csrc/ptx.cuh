@@ -123,4 +123,16 @@ __device__ __forceinline__ void tma_bulk_g2s(uint32_t smem_dst, const void* gmem
                :: "r"(smem_dst), "l"(gmem_src), "r"(bytes), "r"(mbar) : "memory");
 }
 
+// schedule tracing (lz_sched.cuh, B200_LZ_TRACE builds only): device-wide nanosecond clock and the SM of this thread
+__device__ __forceinline__ uint64_t globaltimer_ns() {
+  uint64_t t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+__device__ __forceinline__ uint32_t sm_id() {
+  uint32_t s;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+  return s;
+}
+
 }  // namespace b200
