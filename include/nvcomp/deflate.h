@@ -1,8 +1,18 @@
 /*
- * nvcomp/deflate.h -- Deflate is OUT OF SCOPE for this library (SURVEY.md section 2: not named by the
- * north star).  The symbols exist so the reference's globbed benchmarks and benchmark_hlif.cpp
- * (which names DeflateManager, benchmarks/benchmark_hlif.cpp:207-212) still compile and link; every
- * entry point returns nvcompErrorNotSupported.
+ * nvcomp/deflate.h -- batched Deflate DECOMPRESSION (csrc/deflate.cu).
+ *
+ * A chunk is one raw RFC 1951 stream (zlib wbits = -15, as the reference's deflate_cpu_* examples write it), with a
+ * 32 KB window and no state across chunks.  Bytes after the end of the final block are ignored (zlib leaves them in
+ * unused_data).  A chunk decodes iff zlib 1.3 accepts it and its output fits in its capacity.
+ *   DecompressGetTempSize   256 bytes (one chunk ticket counter); DecompressAsync also runs with temp == nullptr.
+ *   DecompressAsync         chunk i -> out[i] (capacity caps[i]); actual and statuses may be null, actual may alias
+ *                           caps.  Per chunk: nvcompSuccess with exactly actual[i] bytes written, or
+ *                           nvcompErrorCannotDecompress (any structural error, output over the capacity, or a
+ *                           compressed size / capacity >= 2^32) with actual[i] = 0.  Any byte alignment.
+ *   GetDecompressSizeAsync  walks each stream without writing: its decoded length, or 0 if it is rejected.
+ * Compression (the three Compress* entry points) and DeflateManager are not supported: they return / throw
+ * nvcompErrorNotSupported.  They exist so the reference's globbed benchmarks and benchmark_hlif.cpp (which names
+ * DeflateManager, benchmarks/benchmark_hlif.cpp:207-212) compile and link.
  */
 #ifndef NVCOMP_DEFLATE_H
 #define NVCOMP_DEFLATE_H

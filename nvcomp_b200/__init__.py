@@ -9,6 +9,6 @@ for device memory, streams and ``torch.distributed`` plumbing.
 There is no CPU fallback: importing :mod:`nvcomp_b200.batched` (or calling
 :func:`nvcomp_b200.load`) raises if the CUDA library has not been built.
 """
-from ._lib import load, lib_path, FORMATS, Status, Type  # noqa: F401
+from ._lib import load, lib_path, FORMATS, DECODE_ONLY_FORMATS, Status, Type  # noqa: F401
 
-__all__ = ["load", "lib_path", "FORMATS", "Status", "Type"]
+__all__ = ["load", "lib_path", "FORMATS", "DECODE_ONLY_FORMATS", "Status", "Type"]

@@ -10,6 +10,11 @@ _LIB = None
 
 FORMATS = ("LZ4", "Snappy", "Cascaded", "Bitcomp", "ANS")
 
+# formats this library decodes but does not encode (streams from zlib, gzip, Parquet / ORC writers, ...): they export
+# only the three decompression entry points below (include/nvcomp/deflate.h, gzip.h)
+DECODE_ONLY_FORMATS = ("Deflate", "Gzip")
+DECODE_ENTRY_POINTS = ("DecompressGetTempSize", "GetDecompressSizeAsync", "DecompressAsync")
+
 # the six (+2 Ex) entry points every format exports -- SURVEY.md section 8b
 ENTRY_POINTS = (
     "CompressGetTempSize",
@@ -104,6 +109,16 @@ def _declare(lib: C.CDLL) -> None:
         for name, args in sigs.items():
             fn = getattr(lib, f"nvcompBatched{fmt}{name}")
             fn.argtypes = args
+            fn.restype = C.c_int
+    decode_sigs = {
+        "DecompressGetTempSize": [sz, sz, szp],
+        "GetDecompressSizeAsync": [vp, vp, vp, sz, vp],
+        "DecompressAsync": [vp, vp, vp, vp, sz, vp, sz, vp, vp, vp],
+    }
+    for fmt in DECODE_ONLY_FORMATS:
+        for name in DECODE_ENTRY_POINTS:
+            fn = getattr(lib, f"nvcompBatched{fmt}{name}")
+            fn.argtypes = decode_sigs[name]
             fn.restype = C.c_int
 
 

@@ -104,28 +104,39 @@ def empty_batch(n: int, stride: int, device: str | torch.device = "cuda", align:
 
 
 class Codec:
-    """One format's six LLIF entry points, bound to raw pointers."""
+    """One format's six LLIF entry points, bound to raw pointers.  Deflate and Gzip (``_lib.DECODE_ONLY_FORMATS``)
+    have only the decompression half: their compress methods raise NotImplementedError."""
 
     def __init__(self, fmt: str, opts=None):
-        if fmt not in _lib.FORMATS:
+        self.decode_only = fmt in _lib.DECODE_ONLY_FORMATS
+        if fmt not in _lib.FORMATS and not self.decode_only:
             raise ValueError(f"unknown format {fmt}")
+        if self.decode_only and opts is not None:
+            raise ValueError(f"{fmt} is decode-only and takes no options")
         self.fmt = fmt
         self.lib = _lib.load()
-        self.opts = opts if opts is not None else DEFAULT_OPTS[fmt]()
+        self.opts = None if self.decode_only else (opts if opts is not None else DEFAULT_OPTS[fmt]())
 
     def _fn(self, name: str):
         return getattr(self.lib, f"nvcompBatched{self.fmt}{name}")
 
+    def _compress_fn(self, name: str):
+        if self.decode_only:
+            raise NotImplementedError(f"{self.fmt} is decode-only in this library: {name} is not available "
+                                      "(compress on the host, e.g. with zlib, and decode on the GPU)")
+        return self._fn(name)
+
     # --- host-only size queries -------------------------------------------------
     def compress_get_temp_size(self, batch_size: int, max_chunk: int) -> int:
         out = C.c_size_t(0)
-        _check("CompressGetTempSize", self._fn("CompressGetTempSize")(batch_size, max_chunk, self.opts, C.byref(out)))
+        _check("CompressGetTempSize",
+               self._compress_fn("CompressGetTempSize")(batch_size, max_chunk, self.opts, C.byref(out)))
         return out.value
 
     def compress_get_max_output_chunk_size(self, max_chunk: int) -> int:
         out = C.c_size_t(0)
         _check("CompressGetMaxOutputChunkSize",
-               self._fn("CompressGetMaxOutputChunkSize")(max_chunk, self.opts, C.byref(out)))
+               self._compress_fn("CompressGetMaxOutputChunkSize")(max_chunk, self.opts, C.byref(out)))
         return out.value
 
     def decompress_get_temp_size(self, batch_size: int, max_chunk: int) -> int:
@@ -136,7 +147,7 @@ class Codec:
     # --- async device calls -----------------------------------------------------
     def compress_async(self, in_ptrs: int, in_bytes: int, max_chunk: int, batch: int, temp: int,
                        temp_bytes: int, out_ptrs: int, out_bytes: int, stream: int) -> None:
-        _check("CompressAsync", self._fn("CompressAsync")(
+        _check("CompressAsync", self._compress_fn("CompressAsync")(
             in_ptrs, in_bytes, max_chunk, batch, temp, temp_bytes, out_ptrs, out_bytes, self.opts, stream))
 
     def get_decompress_size_async(self, comp_ptrs: int, comp_bytes: int, out_sizes: int, batch: int,

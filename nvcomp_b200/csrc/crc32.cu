@@ -1,12 +1,7 @@
 // crc32.cu -- standard CRC-32 (IEEE 802.3, reflected polynomial 0xEDB88320, the zlib / boost::crc_32_type
 // value) on the GPU: the low-level batched API (reference CHANGELOG.md:51 "Standard CRC32 support and its LLAPI";
 // reference examples/standard_crc_checksum.cpp:94-104 checks it against boost::crc_32_type) and the
-// whole-buffer checksums of the high-level interface (hlif.cu).
-//
-// A CRC is linear over GF(2): with a zero initial register, crc0(A || B) = crc0(A) * x^(8|B|) + crc0(B)
-// (mod P).  So every lane hashes its own contiguous slice byte-table-wise, and slices / pieces are
-// merged with one carry-less modular multiplication each; the 0xFFFFFFFF pre/post conditioning of
-// the standard CRC is added once at the end:  crc32(M) = crc0(M) ^ x^(8|M|) * 0xFFFFFFFF ^ 0xFFFFFFFF.
+// whole-buffer checksums of the high-level interface (hlif.cu).  The warp routine and the method are in crc32.cuh.
 #include "crc32.cuh"
 
 #include "common.cuh"
@@ -18,25 +13,8 @@ __constant__ uint32_t c_crc_table[256];
 __constant__ uint32_t c_crc_x2n[32];      // x^(2^k) mod P, reflected
 
 static void crc_host_tables(uint32_t* table, uint32_t* x2n) {
-  for (uint32_t i = 0; i < 256; ++i) {
-    uint32_t c = i;
-    for (int k = 0; k < 8; ++k) c = (c & 1u) ? (c >> 1) ^ kCrcPoly : c >> 1;
-    table[i] = c;
-  }
-  // x^1 is bit 30 in the reflected representation (x^0 = bit 31)
-  uint32_t p = 1u << 30;
-  x2n[0] = p;
-  for (int k = 1; k < 32; ++k) {
-    // p = p * p mod P
-    uint32_t a = p, b = p, m = 1u << 31, r = 0;
-    while (true) {
-      if (a & m) { r ^= b; if ((a & (m - 1)) == 0) break; }
-      m >>= 1;
-      b = (b & 1u) ? (b >> 1) ^ kCrcPoly : b >> 1;
-    }
-    p = r;
-    x2n[k] = p;
-  }
+  for (uint32_t i = 0; i < 256; ++i) table[i] = crc_table_entry(i);
+  for (int k = 0; k < 32; ++k) x2n[k] = crc_x2n_entry(k);
 }
 
 // constant tables are per device: upload once per device (atomic memo, like ensure_dynamic_smem)
@@ -56,59 +34,6 @@ cudaError_t crc_init_tables() {
   return e;
 }
 
-// a * b mod P (reflected bit order)
-__device__ __forceinline__ uint32_t crc_mulmod(uint32_t a, uint32_t b) {
-  uint32_t r = 0;
-#pragma unroll 4
-  for (int k = 31; k >= 0; --k) {
-    if ((a >> k) & 1u) r ^= b;
-    b = (b & 1u) ? (b >> 1) ^ kCrcPoly : b >> 1;
-  }
-  return r;
-}
-// x^(8 n) mod P
-__device__ __forceinline__ uint32_t crc_x8n(uint64_t n) {
-  uint32_t p = 1u << 31;        // x^0
-  int k = 3;                    // x^(8n) = prod over set bits i of n of x^(2^(i+3))
-  while (n) {
-    if (n & 1ull) p = crc_mulmod(c_crc_x2n[k & 31], p);
-    n >>= 1;
-    ++k;
-  }
-  return p;
-}
-// crc0 of bytes [p, p+n) continuing register c
-__device__ __forceinline__ uint32_t crc_bytes(const uint32_t* __restrict__ table, uint32_t c,
-                                              const uint8_t* __restrict__ p, size_t n) {
-  size_t i = 0;
-  // head up to 4-byte alignment, then word loads
-  for (; i < n && (((uintptr_t)(p + i)) & 3u); ++i) c = table[(c ^ p[i]) & 255u] ^ (c >> 8);
-  for (; i + 4 <= n; i += 4) {
-    const uint32_t w = *(const uint32_t*)(p + i);
-    c ^= w;
-    c = table[c & 255u] ^ (c >> 8);
-    c = table[c & 255u] ^ (c >> 8);
-    c = table[c & 255u] ^ (c >> 8);
-    c = table[c & 255u] ^ (c >> 8);
-  }
-  for (; i < n; ++i) c = table[(c ^ p[i]) & 255u] ^ (c >> 8);
-  return c;
-}
-
-// crc0 of one span by one warp: contiguous slice per lane, merged with x^(8 * bytes after the slice)
-__device__ __forceinline__ uint32_t crc0_warp(const uint32_t* table, const uint8_t* p, size_t n, int lane) {
-  const size_t slice = ((n + 31) / 32 + 3) & ~(size_t)3;
-  const size_t lo = min((size_t)lane * slice, n), hi = min(lo + slice, n);
-  uint32_t c = crc_bytes(table, 0u, p + lo, hi - lo);
-  if (hi < n && c) c = crc_mulmod(crc_x8n(n - hi), c);
-#pragma unroll
-  for (int d = 16; d; d >>= 1) c ^= __shfl_xor_sync(kFull, c, d);
-  return c;
-}
-__device__ __forceinline__ uint32_t crc_finish(uint32_t crc0, uint64_t n) {
-  return crc0 ^ crc_mulmod(crc_x8n(n), 0xffffffffu) ^ 0xffffffffu;
-}
-
 constexpr int kCrcWarps = 8;
 
 // batched: one warp per chunk
@@ -123,8 +48,8 @@ crc32_batch_kernel(const void* const* __restrict__ ptrs, const size_t* __restric
   for (size_t c = (size_t)blockIdx.x * kCrcWarps + (threadIdx.x >> 5); c < batch; c += warps_total) {
     const uint8_t* p = (const uint8_t*)ptrs[c];
     const size_t n = bytes[c];
-    const uint32_t c0 = crc0_warp(s_table, p, n, lane);
-    if (lane == 0) crcs[c] = crc_finish(c0, n);
+    const uint32_t c0 = crc0_warp(s_table, c_crc_x2n, p, n, lane);
+    if (lane == 0) crcs[c] = crc_finish(c_crc_x2n, c0, n);
   }
 }
 
@@ -144,7 +69,7 @@ crc32_pieces_kernel(const uint8_t* __restrict__ data, size_t n_host, const unsig
   for (size_t i = (size_t)blockIdx.x * kCrcWarps + (threadIdx.x >> 5); i < max_pieces; i += warps_total) {
     const size_t lo = i * kCrcPiece;
     uint32_t c0 = 0;
-    if (lo < n) c0 = crc0_warp(s_table, data + lo, min(kCrcPiece, n - lo), lane);
+    if (lo < n) c0 = crc0_warp(s_table, c_crc_x2n, data + lo, min(kCrcPiece, n - lo), lane);
     if (lane == 0) piece_crc0[i] = c0;
   }
 }
@@ -162,13 +87,13 @@ crc32_fold_kernel(const uint32_t* __restrict__ piece_crc0, size_t n_host, const 
   const size_t pieces = (n + kCrcPiece - 1) / kCrcPiece;
   const size_t per = (pieces + blockDim.x - 1) / blockDim.x;
   const size_t p0 = min((size_t)threadIdx.x * per, pieces), p1 = min(p0 + per, pieces);
-  const uint32_t xpiece = crc_x8n(kCrcPiece);
+  const uint32_t xpiece = crc_x8n(c_crc_x2n, kCrcPiece);
   uint32_t c = 0;
   unsigned long long len = 0;
   for (size_t i = p0; i < p1; ++i) {
     const unsigned long long li = min((unsigned long long)kCrcPiece, (unsigned long long)(n - i * kCrcPiece));
     // appending piece i: c = c * x^(8 li) + crc0_i ; li == kCrcPiece except for the very last piece
-    if (c) c = crc_mulmod(li == kCrcPiece ? xpiece : crc_x8n(li), c);
+    if (c) c = crc_mulmod(li == kCrcPiece ? xpiece : crc_x8n(c_crc_x2n, li), c);
     c ^= piece_crc0[i];
     len += li;
   }
@@ -180,13 +105,13 @@ crc32_fold_kernel(const uint32_t* __restrict__ piece_crc0, size_t n_host, const 
     if ((i & (2 * stride - 1)) == 0 && i + stride < blockDim.x) {
       const unsigned long long lr = s_len[i + stride];
       uint32_t cl = s_c[i];
-      if (cl && lr) cl = crc_mulmod(crc_x8n(lr), cl);
+      if (cl && lr) cl = crc_mulmod(crc_x8n(c_crc_x2n, lr), cl);
       s_c[i] = cl ^ s_c[i + stride];
       s_len[i] += lr;
     }
     __syncthreads();
   }
-  if (threadIdx.x == 0) *result = crc_finish(s_c[0], n);
+  if (threadIdx.x == 0) *result = crc_finish(c_crc_x2n, s_c[0], n);
 }
 
 size_t crc_scratch_words(size_t max_bytes) { return (max_bytes + kCrcPiece - 1) / kCrcPiece + 1; }

@@ -511,9 +511,10 @@ std::shared_ptr<nvcompManagerBase> create_manager(const uint8_t* comp_buffer, cu
 }  // namespace nvcomp
 
 // ------------------------------------------------------------------------------------------
-// Out-of-scope formats: LLIF symbols that report nvcompErrorNotSupported (see include/nvcomp/gdeflate.h).
+// Out-of-scope formats: LLIF symbols that report nvcompErrorNotSupported (see include/nvcomp/gdeflate.h).  Deflate
+// and Gzip decompression live in deflate.cu; Deflate compression is not supported.
 // ------------------------------------------------------------------------------------------
-#define B200_UNSUPPORTED_LLIF(FMT)                                                                               \
+#define B200_UNSUPPORTED_COMPRESS(FMT)                                                                           \
   extern "C" {                                                                                                   \
   nvcompStatus_t nvcompBatched##FMT##CompressGetTempSize(size_t, size_t, nvcompBatched##FMT##Opts_t, size_t*) {   \
     return nvcompErrorNotSupported; }                                                                            \
@@ -521,6 +522,10 @@ std::shared_ptr<nvcompManagerBase> create_manager(const uint8_t* comp_buffer, cu
     return nvcompErrorNotSupported; }                                                                            \
   nvcompStatus_t nvcompBatched##FMT##CompressAsync(const void* const*, const size_t*, size_t, size_t, void*, size_t, \
       void* const*, size_t*, nvcompBatched##FMT##Opts_t, cudaStream_t) { return nvcompErrorNotSupported; }        \
+  }
+#define B200_UNSUPPORTED_LLIF(FMT)                                                                               \
+  B200_UNSUPPORTED_COMPRESS(FMT)                                                                                 \
+  extern "C" {                                                                                                   \
   nvcompStatus_t nvcompBatched##FMT##DecompressGetTempSize(size_t, size_t, size_t*) { return nvcompErrorNotSupported; } \
   nvcompStatus_t nvcompBatched##FMT##GetDecompressSizeAsync(const void* const*, const size_t*, size_t*, size_t,    \
       cudaStream_t) { return nvcompErrorNotSupported; }                                                          \
@@ -529,14 +534,5 @@ std::shared_ptr<nvcompManagerBase> create_manager(const uint8_t* comp_buffer, cu
   }
 
 B200_UNSUPPORTED_LLIF(Gdeflate)
-B200_UNSUPPORTED_LLIF(Deflate)
+B200_UNSUPPORTED_COMPRESS(Deflate)
 B200_UNSUPPORTED_LLIF(Zstd)
-
-#include "nvcomp/gzip.h"
-extern "C" {
-nvcompStatus_t nvcompBatchedGzipDecompressGetTempSize(size_t, size_t, size_t*) { return nvcompErrorNotSupported; }
-nvcompStatus_t nvcompBatchedGzipGetDecompressSizeAsync(const void* const*, const size_t*, size_t*, size_t, cudaStream_t) {
-  return nvcompErrorNotSupported; }
-nvcompStatus_t nvcompBatchedGzipDecompressAsync(const void* const*, const size_t*, const size_t*, size_t*, size_t,
-    void* const, size_t, void* const*, nvcompStatus_t*, cudaStream_t) { return nvcompErrorNotSupported; }
-}
