@@ -12,11 +12,11 @@ HDRS      := $(wildcard $(SRC_DIR)/*.cuh) $(wildcard $(SRC_DIR)/*.h) $(wildcard 
 ORACLE_SRCS := $(wildcard oracle/*.c)
 ORACLE_LIB  := oracle/liboracle.so
 
-TESTS_BIN := build/tests/hlif_test
+TESTS_BIN := build/tests/hlif_test build/tests/deflate_hlif_test
 
 # host warp emulator (test infrastructure): the warp-level decode headers compiled with g++, PTX shadowed
 EMU_LIB  := tests/emu/libemu_lz.so
-EMU_SRCS := tests/emu/emu_cuda.cpp tests/emu/emu_lz.cpp tests/emu/emu_inflate.cpp
+EMU_SRCS := tests/emu/emu_cuda.cpp tests/emu/emu_lz.cpp tests/emu/emu_inflate.cpp tests/emu/emu_deflate.cpp
 
 all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(EMU_LIB)
 
@@ -35,7 +35,7 @@ $(LIB): $(OBJS)
 $(ORACLE_LIB): $(ORACLE_SRCS) $(wildcard oracle/*.h)
 	gcc -O3 -march=x86-64-v2 -fPIC -shared -Wall -o $@ $(ORACLE_SRCS) -ldl -lpthread
 
-build/tests/hlif_test: tests/cpp/hlif_test.cu $(LIB) $(HDRS)
+build/tests/%: tests/cpp/%.cu $(LIB) $(HDRS)
 	@mkdir -p build/tests
 	$(NVCC) $(ARCH) -std=c++17 -O2 -Iinclude $< -o $@ -Lnvcomp_b200/lib -lnvcomp -Xlinker '-rpath=$$ORIGIN/../../nvcomp_b200/lib'
 

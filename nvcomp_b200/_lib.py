@@ -8,11 +8,11 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB = None
 
-FORMATS = ("LZ4", "Snappy", "Cascaded", "Bitcomp", "ANS")
+FORMATS = ("LZ4", "Snappy", "Cascaded", "Bitcomp", "ANS", "Deflate")
 
 # formats this library decodes but does not encode (streams from zlib, gzip, Parquet / ORC writers, ...): they export
-# only the three decompression entry points below (include/nvcomp/deflate.h, gzip.h)
-DECODE_ONLY_FORMATS = ("Deflate", "Gzip")
+# only the three decompression entry points below (include/nvcomp/gzip.h)
+DECODE_ONLY_FORMATS = ("Gzip",)
 DECODE_ENTRY_POINTS = ("DecompressGetTempSize", "GetDecompressSizeAsync", "DecompressAsync")
 
 # the six (+2 Ex) entry points every format exports -- SURVEY.md section 8b
@@ -76,8 +76,12 @@ class ANSOpts(C.Structure):
     _fields_ = [("type", C.c_int)]
 
 
+class DeflateOpts(C.Structure):
+    _fields_ = [("algo", C.c_int)]     # 0 high throughput, 1 high compression, 2 entropy only
+
+
 OPTS = {"LZ4": LZ4Opts, "Snappy": SnappyOpts, "Cascaded": CascadedOpts,
-        "Bitcomp": BitcompOpts, "ANS": ANSOpts}
+        "Bitcomp": BitcompOpts, "ANS": ANSOpts, "Deflate": DeflateOpts}
 
 DEFAULT_OPTS = {
     "LZ4": lambda: LZ4Opts(Type.CHAR),
@@ -85,6 +89,7 @@ DEFAULT_OPTS = {
     "Cascaded": lambda: CascadedOpts(4096, Type.INT, 2, 1, 1),
     "Bitcomp": lambda: BitcompOpts(0, Type.UCHAR),
     "ANS": lambda: ANSOpts(0),
+    "Deflate": lambda: DeflateOpts(0),
 }
 
 

@@ -26,7 +26,8 @@ namespace nvcomp {
 namespace detail {
 
 constexpr uint32_t kHlifMagic = 0x3242564eu;   // "NVB2"
-enum FormatId : uint32_t { kFmtLZ4 = 1, kFmtSnappy = 2, kFmtCascaded = 3, kFmtBitcomp = 4, kFmtANS = 5 };
+enum FormatId : uint32_t { kFmtLZ4 = 1, kFmtSnappy = 2, kFmtCascaded = 3, kFmtBitcomp = 4, kFmtANS = 5,
+                        kFmtDeflate = 6 };
 
 struct HlifHeader {
   uint32_t magic;
@@ -89,6 +90,7 @@ B200_BIND(Snappy, nvcompBatchedSnappyOpts_t, kFmtSnappy, 8)
 B200_BIND(Cascaded, nvcompBatchedCascadedOpts_t, kFmtCascaded, 8)
 B200_BIND(Bitcomp, nvcompBatchedBitcompFormatOpts, kFmtBitcomp, 8)
 B200_BIND(ANS, nvcompBatchedANSOpts_t, kFmtANS, 8)
+B200_BIND(Deflate, nvcompBatchedDeflateOpts_t, kFmtDeflate, 8)
 
 static void check(cudaError_t e, const char* what) {
   if (e != cudaSuccess) throw NVCompException(nvcompErrorCudaError, std::string(what) + ": " + cudaGetErrorString(e));
@@ -475,6 +477,7 @@ B200_MANAGER(Snappy, nvcompBatchedSnappyOpts_t)
 B200_MANAGER(Cascaded, nvcompBatchedCascadedOpts_t)
 B200_MANAGER(Bitcomp, nvcompBatchedBitcompFormatOpts)
 B200_MANAGER(ANS, nvcompBatchedANSOpts_t)
+B200_MANAGER(Deflate, nvcompBatchedDeflateOpts_t)
 
 #define B200_UNSUPPORTED_MANAGER(FMT)                                                                             \
   FMT##Manager::FMT##Manager(size_t, const nvcompBatched##FMT##Opts_t&, cudaStream_t, const int, ChecksumPolicy) { \
@@ -483,7 +486,6 @@ B200_MANAGER(ANS, nvcompBatchedANSOpts_t)
   FMT##Manager::~FMT##Manager() = default;
 
 B200_UNSUPPORTED_MANAGER(Gdeflate)
-B200_UNSUPPORTED_MANAGER(Deflate)
 B200_UNSUPPORTED_MANAGER(Zstd)
 
 std::shared_ptr<nvcompManagerBase> create_manager(const uint8_t* comp_buffer, cudaStream_t stream, const int device_id,
@@ -504,6 +506,8 @@ std::shared_ptr<nvcompManagerBase> create_manager(const uint8_t* comp_buffer, cu
       return std::make_shared<BitcompManager>(h.chunk_bytes, o, stream, device_id, policy); }
     case detail::kFmtANS: { nvcompBatchedANSOpts_t o; std::memcpy(&o, h.opts, sizeof(o));
       return std::make_shared<ANSManager>(h.chunk_bytes, o, stream, device_id, policy); }
+    case detail::kFmtDeflate: { nvcompBatchedDeflateOpts_t o; std::memcpy(&o, h.opts, sizeof(o));
+      return std::make_shared<DeflateManager>(h.chunk_bytes, o, stream, device_id, policy); }
     default: throw NVCompException(nvcompErrorInvalidValue, "unknown format id in compressed buffer");
   }
 }
@@ -512,7 +516,7 @@ std::shared_ptr<nvcompManagerBase> create_manager(const uint8_t* comp_buffer, cu
 
 // ------------------------------------------------------------------------------------------
 // Out-of-scope formats: LLIF symbols that report nvcompErrorNotSupported (see include/nvcomp/gdeflate.h).  Deflate
-// and Gzip decompression live in deflate.cu; Deflate compression is not supported.
+// and Gzip live in deflate.cu.
 // ------------------------------------------------------------------------------------------
 #define B200_UNSUPPORTED_COMPRESS(FMT)                                                                           \
   extern "C" {                                                                                                   \
@@ -534,5 +538,4 @@ std::shared_ptr<nvcompManagerBase> create_manager(const uint8_t* comp_buffer, cu
   }
 
 B200_UNSUPPORTED_LLIF(Gdeflate)
-B200_UNSUPPORTED_COMPRESS(Deflate)
 B200_UNSUPPORTED_LLIF(Zstd)
