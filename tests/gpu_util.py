@@ -17,10 +17,9 @@ CANARY = 0x3C
 def _guarded_batch(lens, misalign=0):
     """Output batch whose chunk i may use lens[i] bytes at a 16-byte aligned address + misalign.  Returns the batch and
     the host mask of the bytes the chunks may write."""
-    body = max(list(lens) + [1])
-    slot = (body + misalign + 15) // 16 * 16 + GUARD
-    offsets = GUARD + misalign + slot * np.arange(len(lens), dtype=np.int64)
-    total = GUARD + slot * max(len(lens), 1)
+    slots = [(n + misalign + 15) // 16 * 16 + GUARD for n in lens]       # each chunk its own slot: one huge chunk
+    offsets = GUARD + misalign + np.cumsum([0] + slots[:-1], dtype=np.int64)[:len(lens)]
+    total = GUARD + max(sum(slots), 1)
     host = np.full(total, CANARY, dtype=np.uint8)
     allowed = np.zeros(total, dtype=bool)
     for o, n in zip(offsets, lens):
@@ -40,11 +39,13 @@ def _check_canaries(host, allowed, offsets, what):
                              f"({int(bad[0] - offsets[max(i, 0)])} from chunk {max(i, 0)}), {bad.size} bytes in all")
 
 
-def gpu_decompress(codec: Codec, comp_chunks, caps, misalign=0, want_actual=True, want_status=True):
-    """comp_chunks: list of bytes; caps: list of output capacities.  Returns (outputs, actual, status, out batch)."""
+def gpu_decompress(codec: Codec, comp_chunks, caps, misalign=0, want_actual=True, want_status=True, in_misalign=None,
+                   out_misalign=None):
+    """comp_chunks: list of bytes; caps: list of output capacities.  Inputs sit at 16-byte aligned addresses +
+    in_misalign, outputs + out_misalign (both default to misalign).  Returns (outputs, actual, status, out batch)."""
     caps = [int(c) for c in caps]
-    comp = make_batch(comp_chunks, misalign=misalign)
-    out, allowed = _guarded_batch(caps, misalign)
+    comp = make_batch(comp_chunks, misalign=misalign if in_misalign is None else in_misalign)
+    out, allowed = _guarded_batch(caps, misalign if out_misalign is None else out_misalign)
     actual, status = codec.decompress(comp, out, max_chunk=max(caps + [1]), want_actual=want_actual,
                                       want_status=want_status)
     torch.cuda.synchronize()
