@@ -16,7 +16,8 @@ TESTS_BIN := build/tests/hlif_test build/tests/deflate_hlif_test
 
 # host warp emulator (test infrastructure): the warp-level decode headers compiled with g++, PTX shadowed
 EMU_LIB  := tests/emu/libemu_lz.so
-EMU_SRCS := tests/emu/emu_cuda.cpp tests/emu/emu_lz.cpp tests/emu/emu_inflate.cpp tests/emu/emu_deflate.cpp
+EMU_SRCS := tests/emu/emu_cuda.cpp tests/emu/emu_lz.cpp tests/emu/emu_inflate.cpp tests/emu/emu_deflate.cpp \
+            tests/emu/emu_zstd.cpp
 
 all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(EMU_LIB)
 

@@ -10,9 +10,9 @@ _LIB = None
 
 FORMATS = ("LZ4", "Snappy", "Cascaded", "Bitcomp", "ANS", "Deflate")
 
-# formats this library decodes but does not encode (streams from zlib, gzip, Parquet / ORC writers, ...): they export
-# only the three decompression entry points below (include/nvcomp/gzip.h)
-DECODE_ONLY_FORMATS = ("Gzip",)
+# formats this library decodes but does not encode (streams from zlib, gzip, libzstd, Parquet / ORC writers, ...):
+# the three decompression entry points below are the ones they implement (include/nvcomp/gzip.h, zstd.h)
+DECODE_ONLY_FORMATS = ("Gzip", "Zstd")
 DECODE_ENTRY_POINTS = ("DecompressGetTempSize", "GetDecompressSizeAsync", "DecompressAsync")
 
 # the six (+2 Ex) entry points every format exports -- SURVEY.md section 8b

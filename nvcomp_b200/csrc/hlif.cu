@@ -516,7 +516,7 @@ std::shared_ptr<nvcompManagerBase> create_manager(const uint8_t* comp_buffer, cu
 
 // ------------------------------------------------------------------------------------------
 // Out-of-scope formats: LLIF symbols that report nvcompErrorNotSupported (see include/nvcomp/gdeflate.h).  Deflate
-// and Gzip live in deflate.cu.
+// and Gzip live in deflate.cu; Zstd decompression lives in zstd.cu, Zstd compression is not provided.
 // ------------------------------------------------------------------------------------------
 #define B200_UNSUPPORTED_COMPRESS(FMT)                                                                           \
   extern "C" {                                                                                                   \
@@ -538,4 +538,4 @@ std::shared_ptr<nvcompManagerBase> create_manager(const uint8_t* comp_buffer, cu
   }
 
 B200_UNSUPPORTED_LLIF(Gdeflate)
-B200_UNSUPPORTED_LLIF(Zstd)
+B200_UNSUPPORTED_COMPRESS(Zstd)
