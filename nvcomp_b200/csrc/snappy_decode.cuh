@@ -23,6 +23,88 @@ __device__ __forceinline__ bool snappy_read_preamble(const uint8_t* __restrict__
   return ulen <= 0xffffffffull;
 }
 
+// ---------------------------------------------------------------------------
+// Run-length steps of the direct loop.  Typed run-length data compresses to short elements: a literal of a few bytes
+// (one value), then copies whose offset is the value's width or less.  A step decodes up to 32 such elements at once,
+// one per lane, from a 124-byte register window of input, and never reads the output back:
+//   - element boundaries by pointer doubling over the window (every byte's "next element if this byte were a tag");
+//   - each element is a map from the 8 output bytes before it to the 8 output bytes after it (every new byte is a
+//     byte of the old 8 or a literal constant); a warp scan composes the maps, so every lane learns the 8 bytes in
+//     front of its element, which hold the whole period of a copy with offset <= 8;
+//   - a scan of the output lengths places the elements, and each lane writes its own element with aligned 8-byte
+//     stores.
+// A step takes the longest prefix of elements that are literals of 1..8 bytes or copy-1 / copy-2 elements with
+// offset 1..8, that lie wholly inside the window and pass the checks the serial path makes.  Any other element goes
+// to the serial element code, which also gives the verdict on invalid ones.
+// ---------------------------------------------------------------------------
+constexpr uint32_t kRlWindow = 124;     // bytes of a step's input window (31 whole words, lane 31's is ragged)
+constexpr uint32_t kRlNone = 255;       // position outside the window
+
+// 4 byte-wide indices (0..7 in the low 3 bits of each byte) -> the nibble selector __byte_perm takes
+__device__ __forceinline__ uint32_t rl_nibbles(uint32_t s) {
+  uint32_t u = s & 0x07070707u;
+  u |= u >> 4;
+  return (u & 0xffu) | ((u >> 8) & 0xff00u);
+}
+
+// 0xff in every byte whose top bit is set (a map's constant bytes)
+__device__ __forceinline__ uint32_t rl_const_mask(uint32_t s) { return ((s >> 7) & 0x01010101u) * 0xffu; }
+
+// An 8-byte state map: byte i of the new state is byte s[i] of the old state, or the constant v[i] when s[i] = 0x80.
+struct RlMap {
+  uint32_t s0, s1, v0, v1;
+  // this = this o f (f applies first)
+  __device__ __forceinline__ void after(uint32_t fs0, uint32_t fs1, uint32_t fv0, uint32_t fv1) {
+    const uint32_t n0 = rl_nibbles(s0), n1 = rl_nibbles(s1);
+    const uint32_t m0 = rl_const_mask(s0), m1 = rl_const_mask(s1);
+    const uint32_t gs0 = __byte_perm(fs0, fs1, n0), gs1 = __byte_perm(fs0, fs1, n1);
+    const uint32_t gv0 = __byte_perm(fv0, fv1, n0), gv1 = __byte_perm(fv0, fv1, n1);
+    s0 = (gs0 & ~m0) | (s0 & m0); s1 = (gs1 & ~m1) | (s1 & m1);
+    v0 = (gv0 & ~m0) | (v0 & m0); v1 = (gv1 & ~m1) | (v1 & m1);
+  }
+  __device__ __forceinline__ uint64_t apply(uint64_t st) const {
+    const uint32_t a = (uint32_t)st, b = (uint32_t)(st >> 32);
+    const uint32_t m0 = rl_const_mask(s0), m1 = rl_const_mask(s1);
+    const uint32_t r0 = (__byte_perm(a, b, rl_nibbles(s0)) & ~m0) | (v0 & m0);
+    const uint32_t r1 = (__byte_perm(a, b, rl_nibbles(s1)) & ~m1) | (v1 & m1);
+    return ((uint64_t)r1 << 32) | r0;
+  }
+};
+
+// 8 bytes of x picked by the 8 nibbles of sel
+__device__ __forceinline__ uint64_t rl_perm(uint64_t x, uint32_t sel) {
+  const uint32_t a = (uint32_t)x, b = (uint32_t)(x >> 32);
+  return ((uint64_t)__byte_perm(a, b, sel >> 16) << 32) | __byte_perm(a, b, sel);
+}
+
+// Lane l holds input bytes ip + 4l .. ip + 4l + 3 (little-endian).  Loads stay in the 16-byte granules that hold
+// [in, in + in_n); bytes past them read as 0.
+__device__ __forceinline__ uint32_t rl_window(const uint8_t* __restrict__ in, uint32_t ip, uintptr_t end16,
+                                              uint32_t ul) {
+  const uintptr_t a = (uintptr_t)(in + ip);
+  const uint32_t* w = (const uint32_t*)(a & ~(uintptr_t)3) + ul;
+  const uint32_t x = (uintptr_t)w < end16 ? *w : 0u;
+  const uint32_t y = __shfl_down_sync(kFull, x, 1);
+  return __funnelshift_r(x, y, 8u * (uint32_t)(a & 3u));
+}
+
+// Byte q (< kRlWindow, or kRlNone -> kRlNone) of the per-position table t (4 positions per lane, one per byte).
+__device__ __forceinline__ uint32_t rl_lookup(uint32_t t, uint32_t q) {
+  const uint32_t w = __shfl_sync(kFull, t, (int)((q >> 2) & 31u));
+  return q == kRlNone ? kRlNone : (w >> (8u * (q & 3u))) & 0xffu;
+}
+
+// The 8 output bytes in front of op (byte 7 = out[op - 1]; bytes before out[0] read as 0).  The caller made the
+// warp's stores visible (__syncwarp).
+__device__ __forceinline__ uint64_t rl_reload(const uint8_t* out, uint32_t op, uint32_t ul) {
+  uint32_t b = 0;
+  if (ul < 8u && op + ul >= 8u) b = out[op + ul - 8u];
+  const uint32_t placed = b << (8u * (ul & 3u));
+  const uint32_t lo = __reduce_or_sync(kFull, ul < 4u ? placed : 0u);
+  const uint32_t hi = __reduce_or_sync(kFull, ul - 4u < 4u ? placed : 0u);
+  return ((uint64_t)hi << 32) | lo;
+}
+
 __device__ __forceinline__ bool snappy_decode_chunk(const uint8_t* __restrict__ in, uint32_t in_n,
                                                     uint8_t* out, uint64_t out_cap,
                                                     uint32_t* produced, int lane) {
@@ -33,59 +115,152 @@ __device__ __forceinline__ bool snappy_decode_chunk(const uint8_t* __restrict__ 
   const uint32_t n_out = (uint32_t)ulen;
   uint32_t op = 0;
   const uint32_t ul = (uint32_t)lane;
+  const uintptr_t end16 = ((uintptr_t)(in + in_n) + 15u) & ~(uintptr_t)15u;
+  uint64_t st = 0;                               // the 8 output bytes in front of op
+  uint32_t win = rl_window(in, ip, end16, ul);   // input bytes ip .. ip + kRlWindow
   while (ip < in_n) {
-    if (ip + 32u <= in_n) {
-      // Window path (typed run-length data: a short literal followed by copies of it).  One coalesced 32-byte load
-      // brings the literal element and the copy elements behind it into a register window; when the copy's period
-      // (1, 2, 4 or 8 bytes) lies inside the literal, the whole run -- every following copy-2 element of the window
-      // with the same offset continues it -- is expanded from the window, no load from the output buffer.
-      const uint32_t b = in[ip + ul];
-      const uint32_t tag = __shfl_sync(kFull, b, 0);
-      if ((tag & 3u) == 0u && (tag >> 2) < 8u) {                 // literal of 1..8 bytes
-        const uint32_t ll = (tag >> 2) + 1u;
-        const uint32_t t2 = __shfl_sync(kFull, b, (int)(1u + ll));
-        const uint32_t k2 = t2 & 3u;
-        const uint32_t o_lo = __shfl_sync(kFull, b, (int)(2u + ll)), o_hi = __shfl_sync(kFull, b, (int)(3u + ll));
-        uint32_t off, ml, used;
-        if (k2 == 1u) { off = ((t2 >> 5) << 8) | o_lo; ml = 4u + ((t2 >> 2) & 7u); used = 3u + ll; }
-        else { off = o_lo | (o_hi << 8); ml = (t2 >> 2) + 1u; used = 4u + ll; }
-        if ((k2 == 1u || k2 == 2u) && off != 0u && off <= ll && off <= 8u && (off & (off - 1u)) == 0u) {
-          // lane i inspects the i-th element behind the first copy
-          const uint32_t p = used + 3u * ul;
-          const uint32_t e0 = __shfl_sync(kFull, b, (int)(p & 31u)), e1 = __shfl_sync(kFull, b, (int)((p + 1u) & 31u)),
-                         e2 = __shfl_sync(kFull, b, (int)((p + 2u) & 31u));
-          const bool same = p + 3u <= 32u && (e0 & 3u) == 2u && (e1 | (e2 << 8)) == off;
-          const unsigned m = __ballot_sync(kFull, same);
-          const uint32_t nf = (uint32_t)__ffs((int)~m) - 1u;     // leading run of continuations (< 10)
-          ml += __reduce_add_sync(kFull, ul < nf ? (e0 >> 2) + 1u : 0u);
-          used += 3u * nf;
-          // every element the window shows continues the run and more input follows: look at the next 32 bytes (ten
-          // whole elements) as long as that holds -- a run longer than the ~600 bytes one window spells stays here
-          // instead of taking the read-back copy below for its tail
-          if (nf != 0u && used + 3u > 32u) {
-            while (ip + used + 32u <= in_n) {
-              const uint32_t b2 = in[ip + used + ul];
-              const uint32_t q = 3u * ul;
-              const uint32_t f0 = __shfl_sync(kFull, b2, (int)(q & 31u)), f1 = __shfl_sync(kFull, b2, (int)((q + 1u) & 31u)),
-                             f2 = __shfl_sync(kFull, b2, (int)((q + 2u) & 31u));
-              const bool same2 = ul < 10u && (f0 & 3u) == 2u && (f1 | (f2 << 8)) == off;
-              const uint32_t nf2 = (uint32_t)__ffs((int)~__ballot_sync(kFull, same2)) - 1u;      // <= 10
-              if (nf2 == 0u) break;
-              ml += __reduce_add_sync(kFull, ul < nf2 ? (f0 >> 2) + 1u : 0u);
-              used += 3u * nf2;
-              if (nf2 < 10u || ml > 0x10000u) break;
-            }
-          }
-          if (ll <= n_out - op && ml <= n_out - op - ll) {
-            if (ul - 1u < ll) out[op + ul - 1u] = (uint8_t)b;    // literals: window lanes 1..ll
-            lz_expand_period_from_window(out + op + ll, ml, off, b, 1u + ll - off, ul);
-            op += ll + ml;
-            ip += used;
-            continue;
+    // element 0 of the window: a run element?  (else straight to the serial code)
+    const uint32_t h0 = __shfl_sync(kFull, win, 0);
+    const uint32_t k0 = h0 & 3u;
+    const uint32_t off0 = k0 == 1u ? ((h0 & 0xe0u) << 3) | ((h0 >> 8) & 0xffu) : (h0 >> 8) & 0xffffu;
+    if (k0 == 0u ? (h0 & 0xffu) < 32u : k0 != 3u && off0 - 1u < 8u) {
+      const uint32_t avail = min(in_n - ip, kRlWindow);
+      // nx: for each of this lane's 4 window positions, where the next element starts if an element started there
+      uint32_t nx = 0;
+#pragma unroll
+      for (uint32_t t = 0; t < 4u; ++t) {
+        const uint32_t p = 4u * ul + t, tag = (win >> (8u * t)) & 0xffu, k = tag & 3u;
+        const uint32_t sz = k == 0u ? ((tag >> 2) < 60u ? (tag >> 2) + 2u : kRlNone) : k == 1u ? 2u : k == 2u ? 3u : 5u;
+        nx |= (p + sz < kRlWindow ? p + sz : kRlNone) << (8u * t);
+      }
+      // pointer doubling: j[r] jumps 2^r elements; lane k composes the jumps of the bits of k
+      uint32_t j[5];
+      j[0] = nx;
+#pragma unroll
+      for (int r = 1; r < 5; ++r) {
+        uint32_t nj = 0;
+#pragma unroll
+        for (uint32_t t = 0; t < 4u; ++t) nj |= rl_lookup(j[r - 1], (j[r - 1] >> (8u * t)) & 0xffu) << (8u * t);
+        j[r] = nj;
+      }
+      uint32_t pos = 0;
+#pragma unroll
+      for (int r = 0; r < 5; ++r) {
+        const uint32_t q = rl_lookup(j[r], pos);
+        if ((ul >> r) & 1u) pos = q;
+      }
+      // this lane's element: 9 bytes from pos
+      const uint32_t pw = pos == kRlNone ? 0u : pos;
+      const uint32_t wi = pw >> 2, sh = 8u * (pw & 3u);
+      const uint32_t wa = __shfl_sync(kFull, win, (int)wi), wb = __shfl_sync(kFull, win, (int)((wi + 1u) & 31u)),
+                     wc = __shfl_sync(kFull, win, (int)((wi + 2u) & 31u));
+      const uint32_t t0 = __funnelshift_r(wa, wb, sh), t1 = __funnelshift_r(wb, wc, sh), t2 = wc >> sh;
+      const uint32_t tag = t0 & 0xffu, kind = tag & 3u;
+      uint32_t size, len, off;
+      if (kind == 0u) { len = (tag >> 2) + 1u; size = len + 1u; off = 0u; }
+      else if (kind == 1u) { len = 4u + ((tag >> 2) & 7u); size = 2u; off = ((tag >> 5) << 8) | ((t0 >> 8) & 0xffu); }
+      else if (kind == 2u) { len = (tag >> 2) + 1u; size = 3u; off = (t0 >> 8) & 0xffffu; }
+      else { len = 0u; size = 5u; off = 0u; }
+      const bool run_kind = kind == 0u ? len <= 8u : kind != 3u && off - 1u < 8u;
+      const bool in_win = pos != kRlNone && pos + size <= avail;
+      // place the elements: op_k = op + the output of the elements before this one
+      uint32_t incl = run_kind ? len : 0u;
+#pragma unroll
+      for (uint32_t d = 1; d < 32u; d <<= 1) {
+        const uint32_t x = __shfl_up_sync(kFull, incl, d);
+        if (ul >= d) incl += x;
+      }
+      const uint32_t excl = incl - (run_kind ? len : 0u);
+      const uint32_t opk = op + excl;
+      // the serial path's checks, for this element in stream order (valid for lanes of the prefix)
+      const bool fast = run_kind && in_win && len <= n_out - opk && (kind == 0u || off <= opk);
+      const unsigned fm = __ballot_sync(kFull, fast);
+      const uint32_t nfast = fm == kFull ? 32u : (uint32_t)__ffs((int)~fm) - 1u;
+      // element nfast goes to the serial code unless only the window's end stopped it (the next step takes it)
+      const bool to_serial = pos != kRlNone && pos < avail && (!run_kind || in_win);
+      const bool serial_next = nfast < 32u && ((__ballot_sync(kFull, to_serial) >> nfast) & 1u);
+      if (nfast != 0u) {
+        const uint32_t last = nfast - 1u;
+        const uint32_t used = __shfl_sync(kFull, pos + size, (int)last);
+        const uint32_t made = __shfl_sync(kFull, incl, (int)last);
+        const uint32_t next_win = rl_window(in, ip + used, end16, ul);   // in flight during the stores
+        // the element's map from the 8 bytes before it to the 8 bytes after it
+        const uint32_t o = run_kind && kind != 0u ? off : 1u;
+        uint64_t lit = ((uint64_t)__funnelshift_r(t1, t2, 8u) << 32) | __funnelshift_r(t0, t1, 8u);
+        RlMap f;
+        uint32_t sel8 = 0;                       // nibble i: 8 - off + (i mod off), the copy's bytes from the state
+        {
+          uint32_t c = 0;
+#pragma unroll
+          for (uint32_t i = 0; i < 8u; ++i) {
+            sel8 |= (8u - o + c) << (4u * i);
+            c = c + 1u == o ? 0u : c + 1u;
           }
         }
+        if (kind == 0u) {
+          const uint32_t l = run_kind ? len : 8u;
+          // new byte i = old byte i + l, or literal byte i + l - 8
+          uint32_t a = 0x03020100u + l * 0x01010101u, b = 0x07060504u + l * 0x01010101u;
+          const uint32_t ca = (a >> 3) & 0x01010101u, cb = (b >> 3) & 0x01010101u;
+          f.s0 = (a & ~(ca * 0xffu)) | (ca << 7);
+          f.s1 = (b & ~(cb * 0xffu)) | (cb << 7);
+          const uint64_t v = lit << (8u * (8u - l));
+          f.v0 = (uint32_t)v; f.v1 = (uint32_t)(v >> 32);
+        } else {
+          // new byte i = old byte len + i, or copy byte len + i - 8 = old byte 8 - off + ((len + i - 8) mod off)
+          uint32_t c = (len + 8u * o - 8u) % o, s = 0;
+          f.s0 = f.s1 = 0;
+#pragma unroll
+          for (uint32_t i = 0; i < 8u; ++i) {
+            s = len + i < 8u ? len + i : 8u - o + c;
+            if (i < 4u) f.s0 |= s << (8u * i); else f.s1 |= s << (8u * (i - 4u));
+            c = c + 1u == o ? 0u : c + 1u;
+          }
+          f.v0 = f.v1 = 0;
+        }
+        // inclusive scan: lane k's map takes the 8 bytes before element 0 to the 8 bytes after element k
+#pragma unroll
+        for (uint32_t d = 1; d < 32u; d <<= 1) {
+          const uint32_t a0 = __shfl_up_sync(kFull, f.s0, d), a1 = __shfl_up_sync(kFull, f.s1, d),
+                         b0 = __shfl_up_sync(kFull, f.v0, d), b1 = __shfl_up_sync(kFull, f.v1, d);
+          if (ul >= d) f.after(a0, a1, b0, b1);
+        }
+        const uint64_t after = f.apply(st);
+        uint64_t before = __shfl_up_sync(kFull, after, 1);
+        if (ul == 0u) before = st;
+        st = __shfl_sync(kFull, after, (int)last);
+        if (ul < nfast) {
+          // the element's bytes, 8 at a time from its start (word m + 1 = word m through sel8, for a copy); stored as
+          // aligned 8-byte words, bytewise where a word is shared with a neighbour
+          uint8_t* dst = out + opk;
+          const uint32_t hd = (uint32_t)((uintptr_t)dst & 7u);
+          uint64_t* aw = (uint64_t*)(dst - hd);
+          uint64_t cur = kind == 0u ? lit : rl_perm(before, sel8), prev = 0;
+          const uint32_t nw = (hd + len + 7u) >> 3;
+#pragma unroll 1
+          for (uint32_t m = 0; m < nw; ++m) {
+            const uint64_t w = hd ? (cur << (8u * hd)) | (prev >> (64u - 8u * hd)) : cur;
+            const int jp = (int)(8u * m) - (int)hd;     // element byte at the word's first byte
+            if (jp >= 0 && jp + 8 <= (int)len) {
+              aw[m] = w;
+            } else {
+              uint8_t* bw = (uint8_t*)(aw + m);
+#pragma unroll
+              for (int t = 0; t < 8; ++t)
+                if (jp + t >= 0 && jp + t < (int)len) bw[t] = (uint8_t)(w >> (8 * t));
+            }
+            prev = cur;
+            cur = rl_perm(cur, sel8);
+          }
+        }
+        op += made;
+        ip += used;
+        win = next_win;
+        if (!serial_next) continue;
+        __syncwarp();                            // the serial code may read these bytes back
       }
     }
+    // serial element
     const uint32_t tag = in[ip++];
     uint32_t len, off;
     const uint32_t kind = tag & 3u;
@@ -104,6 +279,9 @@ __device__ __forceinline__ bool snappy_decode_chunk(const uint8_t* __restrict__ 
       warp_copy<true>(out + op, in + ip, len, lane);
       ip += len;
       op += len;
+      __syncwarp();
+      st = rl_reload(out, op, ul);
+      win = rl_window(in, ip, end16, ul);
       continue;
     }
     if (kind == 1) {
@@ -146,6 +324,8 @@ __device__ __forceinline__ bool snappy_decode_chunk(const uint8_t* __restrict__ 
     warp_match_copy(out + op, off, len, lane);
     __syncwarp();
     op += len;
+    st = rl_reload(out, op, ul);
+    win = rl_window(in, ip, end16, ul);
   }
   if (op != n_out) return false;
   *produced = op;
