@@ -205,7 +205,7 @@ __device__ __forceinline__ bool casc_final_rle(const uint8_t* __restrict__ paylo
   };
   const uint32_t* const rw32 = rh.bits ? (const uint32_t*)rwords : (const uint32_t*)payload;
   const uint32_t rmask = rh.bits >= 32u ? 0xffffffffu : ((1u << rh.bits) - 1u);
-  const uint32_t rmin = (uint32_t)rh.minv, rlast = nvals - 1u;
+  const uint32_t rlast = nvals - 1u;
   const uint32_t vnw32 = (uint32_t)(((uint64_t)count * vh.bits + 63u) >> 6) << 1;   // 32-bit words of the two streams
   const uint32_t rnw32 = (uint32_t)(((uint64_t)nvals * rh.bits + 63u) >> 6) << 1;
   const uint32_t stage_s = smem_addr(stage);
@@ -245,9 +245,14 @@ __device__ __forceinline__ bool casc_final_rle(const uint8_t* __restrict__ paylo
     }
     uint32_t len[4];
     unpack32_x4(rw32, k0, rlast, rh.bits, rmask, rnw32, len);
+    bool zero = false;
 #pragma unroll
-    for (int e = 0; e < 4; ++e)
-      len[e] = (k0 + e < nvals) ? min(len[e] + rmin, cap + 1u) : 0u;   // (clipped: no wrap-around in the sums below)
+    for (int e = 0; e < 4; ++e) {
+      // the length is the full 64-bit raw + min, clipped to cap + 1 (no wrap-around in the sums below)
+      len[e] = (k0 + e < nvals) ? (uint32_t)min((uint64_t)len[e] + rh.minv, (uint64_t)cap + 1u) : 0u;
+      zero |= k0 + e < nvals && len[e] == 0u;
+    }
+    if (__any_sync(kFull, zero)) return false;         // a run of length 0
     const uint32_t ltot = len[0] + len[1] + len[2] + len[3];
     const uint32_t lincl = warp_incl_scan<uint32_t>(ltot, lane);
     const uint32_t pos0 = lincl - ltot + lcarry;
@@ -493,14 +498,17 @@ __device__ bool casc_decode_part(const uint8_t* __restrict__ payload, uint32_t p
       for (uint32_t base = 0; base < count; base += 4u * kWarp) {
         const uint32_t k0 = base + 4u * (uint32_t)lane;
         uint32_t len[4];
+        bool zero = false;
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          uint32_t l = 0u;
-          if (k0 + e < count)
-            l = narrow ? (uint32_t)unpack32_at(rw32, k0 + e, rh.bits, rmask, rh.minv)
-                       : (uint32_t)min((unsigned long long)unpack_at(rwords, k0 + e, rh.bits, rh.minv), (unsigned long long)cap + 1ull);
-          len[e] = min(l, cap + 1u);                    // no wrap-around in the sums below
+          uint64_t l = 0u;
+          if (k0 + e < count) {
+            l = narrow ? unpack32_at(rw32, k0 + e, rh.bits, rmask, rh.minv) : unpack_at(rwords, k0 + e, rh.bits, rh.minv);
+            zero |= l == 0u;
+          }
+          len[e] = (uint32_t)min(l, (uint64_t)cap + 1u);   // the full 64-bit length, clipped: no wrap-around below
         }
+        if (__any_sync(kFull, zero)) return false;     // a run of length 0
         const uint32_t p1 = len[0], p2 = p1 + len[1], p3 = p2 + len[2], tot = p3 + len[3];
         const uint32_t incl = warp_incl_scan<uint32_t>(tot, lane);
         const uint32_t ex = incl - tot + carry;

@@ -42,6 +42,10 @@ long oracle_snappy_decompressed_size(const uint8_t* src, size_t n);
 long oracle_snappy_compress(const uint8_t* src, size_t n, uint8_t* dst, size_t cap);
 size_t oracle_snappy_bound(size_t n);
 
+/* Test hook of the Cascaded / Bitcomp / ANS decoders (typed_oracle.c): skip the named rejection rules
+ * (comma-separated; NULL: none) in the calling thread. */
+void oracle_typed_skip_rules(const char* names);
+
 /* codec ids for the threaded batch runner */
 enum { ORACLE_LZ4 = 0, ORACLE_SNAPPY = 1, ORACLE_CASCADED = 2, ORACLE_BITCOMP = 3, ORACLE_ANS = 4,
        ORACLE_LIBLZ4 = 5 /* liblz4.so.1's LZ4_decompress_safe (dlopen), not the port */ };

@@ -12,6 +12,21 @@
 #include <stdlib.h>
 #include <string.h>
 
+/* Every rejection is a named rule (DESIGN.md lists them by format).  oracle_typed_skip_rules() is a test hook: the
+ * rules it names (comma-separated; NULL: none) are not applied in the calling thread, so a test can show that a
+ * malformed stream breaks exactly the rules it is built to break.  A skipped rule can make the oracle read or write past
+ * the stream or the output: only for callers that leave room for that. */
+static __thread const char* skip_rules;
+void oracle_typed_skip_rules(const char* names) { skip_rules = names; }
+static int broken(const char* rule, int cond)
+{
+  if (!cond || !skip_rules) return cond;
+  size_t k = strlen(rule);
+  for (const char* p = skip_rules; (p = strstr(p, rule)) != NULL; p += k)
+    if ((p == skip_rules || p[-1] == ',') && (p[k] == ',' || p[k] == 0)) return 0;
+  return 1;
+}
+
 static uint32_t rd32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
 static uint64_t rd64(const uint8_t* p) { uint64_t v; memcpy(&v, p, 8); return v; }
 static void wr32(uint8_t* p, uint32_t v) { memcpy(p, &v, 4); }
@@ -65,11 +80,11 @@ typedef struct { uint32_t count, bits; uint64_t minv; const uint8_t* words; size
 
 static int read_stream(const uint8_t* p, size_t avail, stream_t* s, size_t* used)
 {
-  if (avail < 16) return -1;
+  if (broken("csc_stream_header_truncated", avail < 16)) return -1;
   s->count = rd32(p); s->bits = rd32(p + 4); s->minv = rd64(p + 8);
-  if (s->bits > 64) return -1;
+  if (broken("csc_stream_bits_above_64", s->bits > 64)) return -1;
   size_t nwords = (size_t)(((uint64_t)s->count * s->bits + 63) / 64);
-  if (16 + 8 * nwords > avail) return -1;
+  if (broken("csc_stream_words_past_partition", 16 + 8 * nwords > avail)) return -1;
   s->words = p + 16; s->nbytes = 8 * nwords;
   *used = 16 + 8 * nwords;
   return 0;
@@ -79,7 +94,7 @@ static long casc_decode_part(const uint8_t* p, size_t nb, uint8_t* out, size_t n
                              size_t cap)
 {
   size_t hdr = 8 * (size_t)D + ((4 * (size_t)D + 7) & ~(size_t)7);
-  if (nb < hdr) return -1;
+  if (broken("csc_part_shorter_than_delta_header", nb < hdr)) return -1;
   const uint8_t* firsts = p;
   const uint8_t* cin = p + 8 * D;
   size_t off = hdr, used;
@@ -89,7 +104,7 @@ static long casc_decode_part(const uint8_t* p, size_t nb, uint8_t* out, size_t n
     off += used;
   }
   if (read_stream(p + off, nb - off, &vals, &used)) return -1;
-  if (vals.count > cap) return -1;
+  if (broken("csc_value_count_above_partition", vals.count > cap)) return -1;
   uint64_t* cur = (uint64_t*)malloc(sizeof(uint64_t) * (cap + 1));
   uint64_t* nxt = (uint64_t*)malloc(sizeof(uint64_t) * (cap + 1));
   int err = 0;
@@ -100,9 +115,10 @@ static long casc_decode_part(const uint8_t* p, size_t nb, uint8_t* out, size_t n
   for (int i = L - 1; i >= 0 && !err; --i) {
     if (i < D) {
       uint32_t c_in = rd32(cin + 4 * i);
-      if (c_in == 0) { if (count != 0) err = 1; }
+      if (c_in == 0) { if (broken("csc_delta_count_zero_with_values", count != 0)) err = 1; }
       else {
-        if (c_in != count + 1 || c_in > cap) { err = 1; break; }
+        if (broken("csc_delta_count_not_values_plus_1", c_in != count + 1) ||
+            broken("csc_delta_count_above_partition", c_in > cap)) { err = 1; break; }
         uint64_t acc = rd64(firsts + 8 * i);
         nxt[0] = trunc_ts(acc, ts);
         for (size_t k = 0; k < count; ++k) { acc += cur[k]; nxt[k + 1] = trunc_ts(acc, ts); }
@@ -111,12 +127,16 @@ static long casc_decode_part(const uint8_t* p, size_t nb, uint8_t* out, size_t n
       }
     }
     if (i < R && !err) {
-      if (runs[i].count != count) { err = 1; break; }
+      if (broken("csc_run_count_not_value_count", runs[i].count != count)) { err = 1; break; }
       size_t total = 0;
       for (size_t k = 0; k < count && !err; ++k) {
         uint64_t len = get_bits(runs[i].words, runs[i].nbytes, (uint64_t)k * runs[i].bits, runs[i].bits, &err)
                        + runs[i].minv;
-        if (len == 0 || total + len > cap) { err = 1; break; }
+        /* len > cap - total, not total + len > cap: a length near 2^64 (raw + min wraps) must not wrap the sum */
+        if (broken("csc_run_zero_length", len == 0) || broken("csc_runs_total_above_partition", len > cap - total)) {
+          err = 1;
+          break;
+        }
         for (uint64_t j = 0; j < len; ++j) nxt[total + j] = cur[k];
         total += len;
       }
@@ -124,7 +144,7 @@ static long casc_decode_part(const uint8_t* p, size_t nb, uint8_t* out, size_t n
       uint64_t* t = cur; cur = nxt; nxt = t;
     }
   }
-  if (!err && count != n_out) err = 1;
+  if (!err && broken("csc_total_not_partition", count != n_out)) err = 1;
   if (!err) for (size_t k = 0; k < count; ++k) store_ts(out + k * ts, cur[k], ts);
   free(cur); free(nxt);
   return err ? -1 : (long)(count * ts);
@@ -132,24 +152,33 @@ static long casc_decode_part(const uint8_t* p, size_t nb, uint8_t* out, size_t n
 
 long oracle_cascaded_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_t cap)
 {
-  if (n < 20 || rd32(src) != CSC_MAGIC) return -1;
+  if (broken("csc_stream_shorter_than_header", n < 20) || broken("csc_magic", rd32(src) != CSC_MAGIC)) return -1;
   uint32_t cfg = rd32(src + 4);
   unsigned type = cfg & 0xff; int R = (cfg >> 8) & 0xff, D = (cfg >> 16) & 0xff;
   unsigned ts = type_size(type);
   uint32_t ulen = rd32(src + 8), P = rd32(src + 12), np = rd32(src + 16);
-  if (!ts || R > 7 || D > 7 || P < 512 || P > 16384 || (P % 8)) return -1;
+  if (broken("csc_type", !ts) || broken("csc_R_above_7", R > 7) || broken("csc_D_above_7", D > 7) ||
+      broken("csc_part_size_below_512", P < 512) || broken("csc_part_size_above_16384", P > 16384) ||
+      broken("csc_part_size_not_multiple_of_8", P % 8))
+    return -1;
+  if (!ts) ts = 1;
   uint32_t tail = ulen % ts, whole = ulen - tail;   /* partitions cover the whole elements */
-  if ((uint64_t)np * P < whole || (np && (uint64_t)(np - 1) * P >= whole)) return -1;
-  if (20 + 4 * ((size_t)np + 1) > n || ulen > cap) return -1;
+  if (broken("csc_num_parts_too_small", (uint64_t)np * P < whole) ||
+      broken("csc_num_parts_too_large", np && (uint64_t)(np - 1) * P >= whole))
+    return -1;
+  if (broken("csc_offset_table_beyond_stream", 20 + 4 * ((size_t)np + 1) > n) || broken("csc_n_above_capacity", ulen > cap))
+    return -1;
   for (uint32_t p = 0; p < np; ++p) {
     uint32_t o0 = rd32(src + 20 + 4 * p), o1 = rd32(src + 20 + 4 * (p + 1));
-    if ((o0 & 7) || o0 > o1 || o1 > n) return -1;
+    if (broken("csc_offset_misaligned", o0 & 7) || broken("csc_offset_decreasing", o0 > o1) ||
+        broken("csc_offset_beyond_stream", o1 > n))
+      return -1;
     uint32_t begin = p * P, nb = whole - begin < P ? whole - begin : P;
     if (casc_decode_part(src + o0, o1 - o0, dst + begin, nb / ts, ts, R, D, P / ts) < 0) return -1;
   }
   if (tail) {   /* trailing bytes: one verbatim word after the last partition */
     uint32_t to = rd32(src + 20 + 4 * np);
-    if ((uint64_t)to + 8 > n) return -1;
+    if (broken("csc_tail_word_missing", (uint64_t)to + 8 > n)) return -1;
     memcpy(dst + whole, src + to, tail);
   }
   return (long)ulen;
@@ -273,13 +302,17 @@ static uint64_t zigzag_ts(uint64_t d, unsigned ts)
 
 long oracle_bitcomp_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_t cap)
 {
-  if (n < 16 || rd32(src) != BTC_MAGIC) return -1;
+  if (broken("btc_stream_shorter_than_header", n < 16) || broken("btc_magic", rd32(src) != BTC_MAGIC)) return -1;
   unsigned algo = rd32(src + 4) & 0xff, type = (rd32(src + 4) >> 8) & 0xff;
   unsigned ts = type_size(type);
   uint32_t ulen = rd32(src + 8), nblocks = rd32(src + 12);
-  if (!ts || algo > 1 || ulen > cap) return -1;
+  if (broken("btc_type", !ts) || broken("btc_algo_above_1", algo > 1) || broken("btc_n_above_capacity", ulen > cap))
+    return -1;
+  if (!ts) ts = 1;
   size_t ne = ulen / ts;
-  if (nblocks != (ne + 127) / 128 || 16 + 2 * (size_t)nblocks > n) return -1;
+  if (broken("btc_nblocks_mismatch", nblocks != (ne + 127) / 128) ||
+      broken("btc_desc_table_beyond_stream", 16 + 2 * (size_t)nblocks > n))
+    return -1;
   size_t off = (16 + 2 * (size_t)nblocks + 7) & ~(size_t)7;
   for (uint32_t b = 0; b < nblocks; ++b) {
     unsigned desc = src[16 + 2 * b] | (src[17 + 2 * b] << 8);
@@ -287,9 +320,9 @@ long oracle_bitcomp_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_
     int err = 0;
     if (algo == 0) {
       unsigned bits = desc & 0xff;
-      if (bits > 64) return -1;
+      if (broken("btc_algo0_bits_above_64", bits > 64)) return -1;
       size_t bytes = 8 + 16 * (size_t)bits;
-      if (off + bytes > n) return -1;
+      if (broken("btc_payload_beyond_stream", off + bytes > n)) return -1;
       uint64_t acc = rd64(src + off);
       for (size_t k = 0; k < nv; ++k) {
         acc += unzigzag(get_bits(src + off + 8, bytes - 8, (uint64_t)k * bits, bits, &err));
@@ -298,11 +331,12 @@ long oracle_bitcomp_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_
       off += bytes;
     } else {
       unsigned nz = desc & 0xff, bits = desc >> 8;
-      if (nz > 128 || bits > 64) return -1;
+      if (broken("btc_algo1_nz_above_128", nz > 128) || broken("btc_algo1_bits_above_64", bits > 64)) return -1;
       size_t bytes = 16 + 8 * (((size_t)nz * bits + 63) / 64);
-      if (off + bytes > n) return -1;
+      if (broken("btc_payload_beyond_stream", off + bytes > n)) return -1;
       uint64_t mlo = rd64(src + off), mhi = rd64(src + off + 8);
-      if ((unsigned)(__builtin_popcountll(mlo) + __builtin_popcountll(mhi)) != nz) return -1;
+      if (broken("btc_algo1_popcount_not_nz", (unsigned)(__builtin_popcountll(mlo) + __builtin_popcountll(mhi)) != nz))
+        return -1;
       unsigned rank = 0;
       for (size_t k = 0; k < nv; ++k) {
         int set = (int)(((k < 64 ? mlo >> k : mhi >> (k - 64))) & 1);
@@ -317,7 +351,7 @@ long oracle_bitcomp_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_
   /* trailing bytes of a chunk whose length is not a multiple of the element size: one verbatim word */
   size_t tail = ulen - ne * ts;
   if (tail) {
-    if (off + 8 > n) return -1;
+    if (broken("btc_tail_word_missing", off + 8 > n)) return -1;
     memcpy(dst + ne * ts, src + off, tail);
   }
   return (long)ulen;
@@ -393,25 +427,36 @@ long oracle_bitcomp_compress(const uint8_t* src, size_t n, uint8_t* dst, size_t 
 
 long oracle_ans_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_t cap)
 {
-  if (n < 16 || rd32(src) != ANS_MAGIC) return -1;
+  if (broken("ans_stream_shorter_than_header", n < 16) || broken("ans_magic", rd32(src) != ANS_MAGIC)) return -1;
   uint32_t ulen = rd32(src + 4), mode = rd32(src + 8), nseg = rd32(src + 12);
-  if (ulen > cap) return -1;
-  if (mode == 1) { if (16 + (size_t)ulen > n) return -1; memcpy(dst, src + 16, ulen); return (long)ulen; }
-  if (mode == 2) { if (n < 17) return -1; memset(dst, src[16], ulen); return (long)ulen; }
-  if (mode != 0 || nseg != (ulen + ANS_SEG - 1) / ANS_SEG) return -1;
-  if (16 + 512 + 4 * ((size_t)nseg + 1) > n) return -1;
+  if (broken("ans_n_above_capacity", ulen > cap)) return -1;
+  if (mode == 1) {
+    if (broken("ans_mode1_short", 16 + (size_t)ulen > n)) return -1;
+    memcpy(dst, src + 16, ulen);
+    return (long)ulen;
+  }
+  if (mode == 2) {
+    if (broken("ans_mode2_short", n < 17)) return -1;
+    memset(dst, src[16], ulen);
+    return (long)ulen;
+  }
+  if (broken("ans_mode_above_2", mode != 0) || broken("ans_nseg_mismatch", nseg != (ulen + ANS_SEG - 1) / ANS_SEG))
+    return -1;
+  if (broken("ans_header_beyond_stream", 16 + 512 + 4 * ((size_t)nseg + 1) > n)) return -1;
   uint32_t cum[257];
   cum[0] = 0;
   for (int s = 0; s < 256; ++s) cum[s + 1] = cum[s] + (src[16 + 2 * s] | (src[17 + 2 * s] << 8));
-  if (cum[256] != ANS_M) return -1;
+  if (broken("ans_freq_sum_not_4096", cum[256] != ANS_M)) return -1;
   static __thread uint8_t sym_of[ANS_M];
   for (int s = 0; s < 256; ++s) {
-    if (cum[s + 1] - cum[s] > 4095) return -1;
-    for (uint32_t k = cum[s]; k < cum[s + 1]; ++k) sym_of[k] = (uint8_t)s;
+    if (broken("ans_single_freq_4096", cum[s + 1] - cum[s] > 4095)) return -1;
+    for (uint32_t k = cum[s]; k < cum[s + 1] && k < ANS_M; ++k) sym_of[k] = (uint8_t)s;
   }
   for (uint32_t sg = 0; sg < nseg; ++sg) {
     uint32_t o0 = rd32(src + 528 + 4 * sg), o1 = rd32(src + 528 + 4 * (sg + 1));
-    if ((o0 & 3) || o0 > o1 || o1 > n || o1 - o0 < 128) return -1;
+    if (broken("ans_seg_offset_misaligned", o0 & 3) || broken("ans_seg_offset_decreasing", o0 > o1) ||
+        broken("ans_seg_offset_past_end", o1 > n) || broken("ans_seg_shorter_than_128", o1 - o0 < 128))
+      return -1;
     uint32_t x[32];
     for (int l = 0; l < 32; ++l) x[l] = rd32(src + o0 + 4 * l);
     const uint8_t* words = src + o0 + 128;
@@ -425,13 +470,13 @@ long oracle_ans_decompress(const uint8_t* src, size_t n, uint8_t* dst, size_t ca
       dst[begin + i] = (uint8_t)s;
       x[l] = (cum[s + 1] - cum[s]) * (x[l] >> 12) + slot - cum[s];
       if (x[l] < ANS_L) {
-        if (wpos >= nwords) return -1;
+        if (broken("ans_words_exhausted", wpos >= nwords)) return -1;
         x[l] = (x[l] << 16) | (uint32_t)(words[2 * wpos] | (words[2 * wpos + 1] << 8));
         ++wpos;
       }
     }
-    if (nwords - wpos > 1) return -1;
-    for (int l = 0; l < 32; ++l) if (x[l] != ANS_L) return -1;
+    if (broken("ans_two_leftover_words", nwords - wpos > 1)) return -1;
+    for (int l = 0; l < 32; ++l) if (broken("ans_final_state_not_L", x[l] != ANS_L)) return -1;
   }
   return (long)ulen;
 }

@@ -39,29 +39,39 @@ def _check_canaries(host, allowed, offsets, what):
                              f"({int(bad[0] - offsets[max(i, 0)])} from chunk {max(i, 0)}), {bad.size} bytes in all")
 
 
-def gpu_decompress(codec: Codec, comp_chunks, caps, misalign=0, want_actual=True, want_status=True, in_misalign=None,
-                   out_misalign=None):
-    """comp_chunks: list of bytes; caps: list of output capacities.  Inputs sit at 16-byte aligned addresses +
-    in_misalign, outputs + out_misalign (both default to misalign).  Returns (outputs, actual, status, out batch)."""
+def guarded_decompress(launch, what: str, comp_chunks, caps, in_misalign=0, out_misalign=0):
+    """Run a decoder into guarded outputs and check them.  launch(comp batch, out batch, max capacity) enqueues the
+    decode and returns its (actual, status) tensors (either may be None).  Inputs sit at 16-byte aligned addresses +
+    in_misalign, outputs + out_misalign.  Returns (outputs, actual, status, out batch)."""
     caps = [int(c) for c in caps]
-    comp = make_batch(comp_chunks, misalign=misalign if in_misalign is None else in_misalign)
-    out, allowed = _guarded_batch(caps, misalign if out_misalign is None else out_misalign)
-    actual, status = codec.decompress(comp, out, max_chunk=max(caps + [1]), want_actual=want_actual,
-                                      want_status=want_status)
+    comp = make_batch(comp_chunks, misalign=in_misalign)
+    out, allowed = _guarded_batch(caps, out_misalign)
+    actual, status = launch(comp, out, max(caps + [1]))
     torch.cuda.synchronize()
-    a = actual.cpu().numpy() if actual is not None else None
-    s = status.cpu().numpy() if status is not None else None
+    a = actual.cpu().numpy()[:len(caps)] if actual is not None else None
+    s = status.cpu().numpy()[:len(caps)] if status is not None else None
     host = out.slab.cpu().numpy()
-    _check_canaries(host, allowed, out.offsets, f"{codec.fmt} decompress")
+    _check_canaries(host, allowed, out.offsets, what)
     if a is not None and s is not None:
         for i, (o, cap) in enumerate(zip(out.offsets, caps)):
             if s[i] == 0:
-                assert a[i] <= cap, (codec.fmt, i, a[i], cap)
+                assert a[i] <= cap, (what, i, a[i], cap)
                 rest = host[o + int(a[i]):o + cap]
-                assert (rest == FILL).all(), \
-                    f"{codec.fmt} decompress: chunk {i} wrote past actual={int(a[i])} (cap {cap})"
-    sizes = a if a is not None else np.asarray(caps)
+                assert (rest == FILL).all(), f"{what}: chunk {i} wrote past actual={int(a[i])} (cap {cap})"
+    sizes = np.maximum(a, 0) if a is not None else np.asarray(caps)
     return out.to_host(sizes), a, s, out
+
+
+def gpu_decompress(codec: Codec, comp_chunks, caps, misalign=0, want_actual=True, want_status=True, in_misalign=None,
+                   out_misalign=None):
+    """comp_chunks: list of bytes; caps: list of output capacities, through the codec's DecompressAsync.  Inputs sit at
+    16-byte aligned addresses + in_misalign, outputs + out_misalign (both default to misalign).  Returns (outputs,
+    actual, status, out batch)."""
+    def launch(comp, out, max_chunk):
+        return codec.decompress(comp, out, max_chunk=max_chunk, want_actual=want_actual, want_status=want_status)
+    return guarded_decompress(launch, f"{codec.fmt} decompress", comp_chunks, caps,
+                              misalign if in_misalign is None else in_misalign,
+                              misalign if out_misalign is None else out_misalign)
 
 
 def gpu_compress(codec: Codec, raw_chunks, misalign=0, out_misalign=0):

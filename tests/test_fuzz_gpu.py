@@ -1,6 +1,7 @@
 """-m gpu: robustness.  Random garbage and bit-flipped valid streams must never fault or hang; every chunk
 ends with status Success (and then the exact size) or CannotDecompress with size 0 (reference
-CHANGELOG.md:160-164: undecodable input yields size 0 + an error status, never an illegal access).
+CHANGELOG.md:160-164: undecodable input yields size 0 + an error status, never an illegal access).  For Cascaded,
+Bitcomp and ANS the verdict, size and bytes must be the oracle's.
 tools: run this file under `compute-sanitizer --tool memcheck` to check for out-of-bounds accesses."""
 import numpy as np
 import pytest
@@ -20,7 +21,7 @@ def _codec(kind):
 
 
 @pytest.mark.parametrize("kind", ["LZ4", "Snappy", "Cascaded", "Bitcomp", "ANS"])
-def test_garbage_and_bitflips(kind):
+def test_garbage_and_bitflips(kind, oracle):
     from gpu_util import gpu_compress, gpu_decompress
     rng = np.random.default_rng(2024)
     codec = _codec(kind)
@@ -50,3 +51,8 @@ def test_garbage_and_bitflips(kind):
             assert actual[i] <= cap
         if e is not None:
             assert status[i] == 0 and outs[i] == e, (kind, i)
+        if kind in ("Cascaded", "Bitcomp", "ANS"):
+            # the typed formats: the oracle's verdict and bytes on every chunk
+            w = oracle.decompress(kind.lower(), c, cap)
+            assert (int(status[i]), int(actual[i])) == ((12, 0) if w is None else (0, len(w))), (kind, i)
+            assert w is None or outs[i] == w, (kind, i)

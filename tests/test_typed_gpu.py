@@ -134,7 +134,12 @@ def test_typed_malformed(kind, oracle):
     outs, actual, status, _ = gpu_decompress(codec, bad + [good], caps + [len(raw)])
     for i in range(5):
         assert status[i] == 12 and actual[i] == 0, (kind, i, status[i], actual[i])
-    assert status[5] in (0, 12)      # corrupted payload: either detected or decoded to garbage, never a fault
+    # corrupted payload: the oracle's verdict, and its bytes when it decodes
+    want = oracle.decompress(kind.lower(), bytes(corrupt), len(raw))
+    if want is None:
+        assert status[5] == 12 and actual[5] == 0, (kind, status[5], actual[5])
+    else:
+        assert status[5] == 0 and outs[5] == want, (kind, status[5], actual[5])
     assert status[6] == 0 and outs[6] == raw
 
 

@@ -68,11 +68,10 @@ def _stream_hdr(vals: list[int], use_bp: bool, signed: bool, ts: int, raw_bits: 
     return (n, (hi - lo).bit_length(), lo & M64)
 
 
-def cascaded_partition(vals: list[int], ts: int, type_signed: bool, R: int, D: int, use_bp: bool) -> dict:
-    """Layer i (i < max(R, D)): run-length encode if i < R (values go on, lengths become run stream i), then
+def cascaded_layers(vals: list[int], ts: int, R: int, D: int) -> tuple[list[int], list[int], list[list[int]], list[int]]:
+    """Layer i (i < max(R, D)): run-length encode if i < R (values go on, lengths become run list i), then
     delta-encode if i < D (the first value is kept in first[i], the element count entering the layer in cnt_in[i];
-    deltas wrap modulo 2^(8*ts)).  The values left at the end are the value stream, bit-packed in the type's own
-    signedness when no delta layer ran, signed after one."""
+    deltas wrap modulo 2^(8*ts)).  Returns (first, cnt_in, run lengths per layer, the values left at the end)."""
     mask = (1 << (8 * ts)) - 1
     cur = list(vals)
     runs, first, cnt_in = [], [], []
@@ -82,12 +81,20 @@ def cascaded_partition(vals: list[int], ts: int, type_signed: bool, R: int, D: i
             for v, g in groupby(cur):
                 vs.append(v)
                 ls.append(sum(1 for _ in g))
-            runs.append(_stream_hdr(ls, use_bp, False, 2, 16))
+            runs.append(ls)
             cur = vs
         if i < D:
             first.append(cur[0] if cur else 0)
             cnt_in.append(len(cur))
             cur = [(b - a) & mask for a, b in zip(cur, cur[1:])]
+    return first, cnt_in, runs, cur
+
+
+def cascaded_partition(vals: list[int], ts: int, type_signed: bool, R: int, D: int, use_bp: bool) -> dict:
+    """cascaded_layers(), then every run list is a stream of 16-bit unsigned lengths and the values left at the end
+    are the value stream, bit-packed in the type's own signedness when no delta layer ran, signed after one."""
+    first, cnt_in, run_lists, cur = cascaded_layers(vals, ts, R, D)
+    runs = [_stream_hdr(ls, use_bp, False, 2, 16) for ls in run_lists]
     vals_hdr = _stream_hdr(cur, use_bp, D > 0 or type_signed, ts, 8 * ts)
     size = 8 * D + _r8(4 * D) + sum(16 + 8 * _words(c, b) for c, b, _ in runs + [vals_hdr])
     return {"first": first, "cnt_in": cnt_in, "runs": runs, "vals": vals_hdr, "size": size, "pad": 0}
@@ -226,26 +233,32 @@ def ans_freq(data: bytes) -> tuple[int, list[int]]:
     return len(hist), freq
 
 
-def ans_segment_words(seg: bytes, freq: list[int]) -> int:
-    """16-bit renormalisation words of one segment: 32 interleaved rANS states (symbol i -> state i % 32), each
-    starting at L = 2^16, encoded from the last symbol back; a state emits a word before coding a symbol of frequency
+def ans_encode_segment(seg: bytes, freq: list[int], start: list[int] | None = None) -> tuple[list[int], list[int]]:
+    """(32 initial decoder states, 16-bit renormalisation words in the order the decoder reads them) of one segment:
+    32 interleaved rANS states (symbol i -> state i % 32), each starting at `start` (default L = 2^16, the state the
+    decoder must end in), encoded from the last symbol back; a state emits a word before coding a symbol of frequency
     f when it is >= f << 20."""
     cum = [0] * 256
     acc = 0
     for s in range(256):
         cum[s] = acc
         acc += freq[s]
-    x = [ANS_L] * 32
-    nw = 0
+    x = list(start) if start else [ANS_L] * 32
+    words = []
     for i in range(len(seg) - 1, -1, -1):
         s = seg[i]
         f = freq[s]
         v = x[i & 31]
         if v >= f << 20:
+            words.append(v & 0xFFFF)
             v >>= 16
-            nw += 1
         x[i & 31] = ((v // f) << 12) + v % f + cum[s]
-    return nw
+    return x, words[::-1]
+
+
+def ans_segment_words(seg: bytes, freq: list[int]) -> int:
+    """Renormalisation words of one segment (ans_encode_segment)."""
+    return len(ans_encode_segment(seg, freq)[1])
 
 
 def ans_model(data: bytes) -> dict:
