@@ -16,13 +16,15 @@ ORACLE_LIB  := oracle/liboracle.so
 TESTS_BIN := build/tests/hlif_test build/tests/deflate_hlif_test
 # kernels over the warp-level ANS device API (include/nvcomp/device/ans.cuh), loaded by the tests with ctypes
 ANS_DEVICE_LIB := build/tests/libans_device.so
+# kernels over the warp-level Bitcomp device API (include/nvcomp/device/bitcomp.cuh), loaded the same way
+BITCOMP_DEVICE_LIB := build/tests/libbitcomp_device.so
 
 # host warp emulator (test infrastructure): the warp-level decode headers compiled with g++, PTX shadowed
 EMU_LIB  := tests/emu/libemu_lz.so
 EMU_SRCS := tests/emu/emu_cuda.cpp tests/emu/emu_lz.cpp tests/emu/emu_inflate.cpp tests/emu/emu_deflate.cpp \
             tests/emu/emu_zstd.cpp
 
-all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(ANS_DEVICE_LIB) $(EMU_LIB)
+all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(ANS_DEVICE_LIB) $(BITCOMP_DEVICE_LIB) $(EMU_LIB)
 
 $(EMU_LIB): $(EMU_SRCS) $(wildcard tests/emu/*.h) $(wildcard tests/emu/*.cuh) $(HDRS)
 	g++ -std=c++17 -O2 -g -fPIC -shared -Wall -Wno-unknown-pragmas -Wno-unused-function \
@@ -47,6 +49,11 @@ $(ANS_DEVICE_LIB): tests/cpp/ans_device_kernels.cu $(HDRS)
 	@mkdir -p build/tests
 	$(NVCC) $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -shared -Xptxas -v $< -o $@ \
 	    2> build/tests/libans_device.ptxas.log || (cat build/tests/libans_device.ptxas.log; exit 1)
+
+$(BITCOMP_DEVICE_LIB): tests/cpp/bitcomp_device_kernels.cu $(HDRS)
+	@mkdir -p build/tests
+	$(NVCC) $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -shared -Xptxas -v $< -o $@ \
+	    2> build/tests/libbitcomp_device.ptxas.log || (cat build/tests/libbitcomp_device.ptxas.log; exit 1)
 
 clean:
 	rm -rf $(BUILD_DIR) $(LIB) $(ORACLE_LIB)
