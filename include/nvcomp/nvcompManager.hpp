@@ -59,8 +59,10 @@ struct DecompressionConfig
   /* upper bound of the compressed buffer's size (header total, or the compression config's bound): sizes the
    * checksum pass over the compressed payload */
   size_t comp_bytes_bound;
-  /* pinned host status of the last decompress() issued with this config (nvcompSuccess,
-   * nvcompErrorCannotDecompress or nvcompErrorBadChecksum); valid after a stream sync */
+  /* pinned host status of the last decompress() issued with this config; valid after a stream sync.
+   * nvcompSuccess: every chunk decoded to exactly its slot of the output (and, when verified, both checksums match);
+   * nvcompErrorCannotDecompress: some chunk failed to decode or decoded to fewer or more bytes than its slot;
+   * nvcompErrorBadChecksum: every chunk decoded but a stored checksum disagrees */
   nvcompStatus_t* get_status() const;
   std::shared_ptr<detail::StatusHolder> status;
 };

@@ -16,7 +16,9 @@
 #include <cstddef>
 #include <cstring>
 #include <memory>
+#include <new>
 #include <string>
+#include <vector>
 
 #include "common.cuh"
 #include "crc32.cuh"
@@ -54,7 +56,10 @@ struct StatusHolder {
 struct FormatBinding {
   uint32_t format = 0;
   uint8_t opts[24] = {0};
-  size_t align = 8;
+  // chunk sizes must be a multiple of this, so that every chunk pointer the manager derives (input, output, container)
+  // keeps the alignment the low-level decoder requires: the typed codecs reject chunk pointers that are not 8-byte
+  // aligned and outputs not aligned to the element size
+  size_t chunk_multiple = 1;
   nvcompStatus_t (*comp_temp)(const FormatBinding&, size_t, size_t, size_t*) = nullptr;
   nvcompStatus_t (*comp_max)(const FormatBinding&, size_t, size_t*) = nullptr;
   nvcompStatus_t (*comp)(const FormatBinding&, const void* const*, const size_t*, size_t, size_t, void*, size_t,
@@ -67,11 +72,11 @@ struct FormatBinding {
 template <class Opts>
 static Opts opts_of(const FormatBinding& b) { Opts o; std::memcpy(&o, b.opts, sizeof(Opts)); return o; }
 
-#define B200_BIND(FMT, OPTS, ID, ALIGN)                                                                      \
+#define B200_BIND(FMT, OPTS, ID, MULTIPLE)                                                                   \
   static FormatBinding bind_##FMT(const OPTS& o) {                                                           \
     static_assert(sizeof(OPTS) <= 24, "opts blob");                                                         \
     FormatBinding b;                                                                                         \
-    b.format = ID; b.align = ALIGN;                                                                          \
+    b.format = ID; b.chunk_multiple = MULTIPLE;                                                              \
     std::memcpy(b.opts, &o, sizeof(OPTS));                                                                   \
     b.comp_temp = [](const FormatBinding& f, size_t n, size_t m, size_t* t) {                                \
       return nvcompBatched##FMT##CompressGetTempSize(n, m, opts_of<OPTS>(f), t); };                          \
@@ -85,12 +90,12 @@ static Opts opts_of(const FormatBinding& b) { Opts o; std::memcpy(&o, b.opts, si
     return b;                                                                                                \
   }
 
-B200_BIND(LZ4, nvcompBatchedLZ4Opts_t, kFmtLZ4, 8)
-B200_BIND(Snappy, nvcompBatchedSnappyOpts_t, kFmtSnappy, 8)
-B200_BIND(Cascaded, nvcompBatchedCascadedOpts_t, kFmtCascaded, 8)
-B200_BIND(Bitcomp, nvcompBatchedBitcompFormatOpts, kFmtBitcomp, 8)
-B200_BIND(ANS, nvcompBatchedANSOpts_t, kFmtANS, 8)
-B200_BIND(Deflate, nvcompBatchedDeflateOpts_t, kFmtDeflate, 8)
+B200_BIND(LZ4, nvcompBatchedLZ4Opts_t, kFmtLZ4, 1)
+B200_BIND(Snappy, nvcompBatchedSnappyOpts_t, kFmtSnappy, 1)
+B200_BIND(Cascaded, nvcompBatchedCascadedOpts_t, kFmtCascaded, nvcompCascadedRequiredAlignment)
+B200_BIND(Bitcomp, nvcompBatchedBitcompFormatOpts, kFmtBitcomp, nvcompBitcompRequiredAlignment)
+B200_BIND(ANS, nvcompBatchedANSOpts_t, kFmtANS, 1)
+B200_BIND(Deflate, nvcompBatchedDeflateOpts_t, kFmtDeflate, 1)
 
 static void check(cudaError_t e, const char* what) {
   if (e != cudaSuccess) throw NVCompException(nvcompErrorCudaError, std::string(what) + ": " + cudaGetErrorString(e));
@@ -220,6 +225,8 @@ struct ManagerImpl {
   ManagerImpl(const FormatBinding& f, size_t chunk_size, cudaStream_t s, int dev, ChecksumPolicy p)
       : fmt(f), chunk(chunk_size), stream(s), device(dev), policy(p) {
     if (chunk_size == 0) throw NVCompException(nvcompErrorInvalidValue, "chunk size must be positive");
+    if (chunk_size % fmt.chunk_multiple != 0)
+      throw NVCompException(nvcompErrorInvalidValue, "chunk size must be a multiple of the format's required alignment");
     size_t probe = 0;
     check(fmt.comp_max(fmt, chunk, &probe), "invalid format options / chunk size");
   }
@@ -355,11 +362,13 @@ struct ManagerImpl {
       throw NVCompException(nvcompErrorCannotVerifyChecksums, "checksums requested but absent from the buffer");
     // the header is untrusted input: every field the pointer setup uses is checked against the others
     size_t probe = 0;
-    if (h.chunk_bytes == 0 || fmt.comp_max(fmt, (size_t)h.chunk_bytes, &probe) != nvcompSuccess)
+    if (h.chunk_bytes == 0 || h.chunk_bytes % fmt.chunk_multiple != 0 ||
+        fmt.comp_max(fmt, (size_t)h.chunk_bytes, &probe) != nvcompSuccess)
       throw NVCompException(nvcompErrorInvalidValue, "corrupt header: chunk size");
     const uint64_t want_chunks = h.uncompressed_bytes == 0 ? 0 : (h.uncompressed_bytes + h.chunk_bytes - 1) / h.chunk_bytes;
     if ((uint64_t)h.num_chunks != want_chunks || h.total_bytes < kHeaderBytes + 8ull * h.num_chunks)
       throw NVCompException(nvcompErrorInvalidValue, "corrupt header: chunk count");
+    check_size_table(comp, h);
     DecompressionConfig d;
     d.decomp_data_size = h.uncompressed_bytes;
     d.num_chunks = h.num_chunks;
@@ -370,6 +379,36 @@ struct ManagerImpl {
                                        crc_span(d.decomp_data_size, d.comp_bytes_bound));
     if (L.total > required_scratch) required_scratch = L.total;
     return d;
+  }
+
+  // The size table is untrusted as well: every chunk pointer and the compressed-payload checksum pass are derived
+  // from it, so every chunk must fit the format's bound and the chunks must end exactly at total_bytes.  The bound is
+  // the one of the options stored in the header, which the chunks were written with: for Cascaded and Bitcomp it
+  // depends on them, and this manager's own options only matter for compression (the decoders read the streams).
+  void check_size_table(const uint8_t* comp, const HlifHeader& h) {
+    FormatBinding stored = fmt;
+    std::memcpy(stored.opts, h.opts, sizeof(stored.opts));
+    size_t max_out = 0;
+    if (stored.comp_max(stored, (size_t)h.chunk_bytes, &max_out) != nvcompSuccess)
+      throw NVCompException(nvcompErrorInvalidValue, "corrupt header: format options");
+    std::vector<uint64_t> sizes;
+    try {
+      sizes.resize(h.num_chunks);
+    } catch (const std::bad_alloc&) {
+      throw NVCompException(nvcompErrorInternal, "no host memory for the size table");
+    }
+    if (h.num_chunks) {
+      check(cudaMemcpyAsync(sizes.data(), comp + kHeaderBytes, 8 * sizes.size(), cudaMemcpyDeviceToHost, stream),
+            "size table read");
+      check(cudaStreamSynchronize(stream), "size table sync");
+    }
+    uint64_t total = kHeaderBytes + 8ull * h.num_chunks;     // no overflow: num_chunks < 2^32, each size <= max_out
+    for (const uint64_t s : sizes) {
+      if (s > max_out) throw NVCompException(nvcompErrorInvalidValue, "corrupt size table: chunk above the format's bound");
+      total += (s + 7) & ~7ull;
+    }
+    if (total != h.total_bytes)
+      throw NVCompException(nvcompErrorInvalidValue, "corrupt size table: chunks do not end at total_bytes");
   }
 
   DecompressionConfig configure_decompression(const CompressionConfig& c) {
@@ -412,24 +451,26 @@ struct ManagerImpl {
       verify = 1;
     }
     if (cfg.status && cfg.status->host)
-      hlif_reduce_status_launch(statuses, nc, comp, sums, verify, cfg.status->host);
+      hlif_reduce_status_launch(statuses, actual, caps, nc, comp, sums, verify, cfg.status->host);
     check(cudaGetLastError(), "decompress launch");
   }
 
-  void hlif_reduce_status_launch(const nvcompStatus_t* statuses, size_t nc, const uint8_t* comp, const uint32_t* sums,
-                                 int verify, nvcompStatus_t* host);
+  void hlif_reduce_status_launch(const nvcompStatus_t* statuses, const size_t* actual, const size_t* caps, size_t nc,
+                                 const uint8_t* comp, const uint32_t* sums, int verify, nvcompStatus_t* host);
 
   size_t get_compressed_output_size(const uint8_t* comp) { return read_header(comp).total_bytes; }
 };
 
+// a chunk fails unless it decodes to exactly its slot (a valid stream may decode to fewer bytes than the capacity);
 // verification only applies when the buffer carries checksums (flag read on the device)
-__global__ void hlif_reduce_status_flagged(const nvcompStatus_t* statuses, size_t num_chunks, const uint8_t* comp_buffer,
-                                           const uint32_t* sums, int verify, nvcompStatus_t* host_status) {
+__global__ void hlif_reduce_status_flagged(const nvcompStatus_t* statuses, const size_t* actual, const size_t* caps,
+                                           size_t num_chunks, const uint8_t* comp_buffer, const uint32_t* sums,
+                                           int verify, nvcompStatus_t* host_status) {
   __shared__ int s_bad;
   if (threadIdx.x == 0) s_bad = 0;
   __syncthreads();
   for (size_t i = threadIdx.x; i < num_chunks; i += blockDim.x)
-    if (statuses[i] != nvcompSuccess) s_bad = 1;
+    if (statuses[i] != nvcompSuccess || actual[i] != caps[i]) s_bad = 1;
   __syncthreads();
   if (threadIdx.x == 0) {
     nvcompStatus_t st = s_bad ? nvcompErrorCannotDecompress : nvcompSuccess;
@@ -441,9 +482,10 @@ __global__ void hlif_reduce_status_flagged(const nvcompStatus_t* statuses, size_
   }
 }
 
-void ManagerImpl::hlif_reduce_status_launch(const nvcompStatus_t* statuses, size_t nc, const uint8_t* comp,
-                                            const uint32_t* sums, int verify, nvcompStatus_t* host) {
-  hlif_reduce_status_flagged<<<1, 256, 0, stream>>>(statuses, nc, comp, sums, verify, host);
+void ManagerImpl::hlif_reduce_status_launch(const nvcompStatus_t* statuses, const size_t* actual, const size_t* caps,
+                                            size_t nc, const uint8_t* comp, const uint32_t* sums, int verify,
+                                            nvcompStatus_t* host) {
+  hlif_reduce_status_flagged<<<1, 256, 0, stream>>>(statuses, actual, caps, nc, comp, sums, verify, host);
 }
 
 }  // namespace detail
