@@ -20,6 +20,8 @@ ANS_DEVICE_LIB := build/tests/libans_device.so
 BITCOMP_DEVICE_LIB := build/tests/libbitcomp_device.so
 # kernels over the warp-level Cascaded device API (include/nvcomp/device/cascaded.cuh), loaded the same way
 CASCADED_DEVICE_LIB := build/tests/libcascaded_device.so
+# kernels over the warp-level LZ4 and Snappy device APIs (include/nvcomp/device/{lz4,snappy}.cuh), loaded the same way
+LZ_DEVICE_LIB := build/tests/liblz_device.so
 # extern "C" dispatch onto the C++ managers (nvcomp::*Manager, create_manager), loaded the same way
 HLIF_SHIM_LIB := build/tests/libhlif_shim.so
 
@@ -28,9 +30,9 @@ EMU_LIB  := tests/emu/libemu_lz.so
 EMU_SRCS := tests/emu/emu_cuda.cpp tests/emu/emu_lz.cpp tests/emu/emu_inflate.cpp tests/emu/emu_deflate.cpp \
             tests/emu/emu_zstd.cpp
 
-all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(ANS_DEVICE_LIB) $(BITCOMP_DEVICE_LIB) $(CASCADED_DEVICE_LIB) $(HLIF_SHIM_LIB) $(EMU_LIB)
+all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(ANS_DEVICE_LIB) $(BITCOMP_DEVICE_LIB) $(CASCADED_DEVICE_LIB) $(LZ_DEVICE_LIB) $(HLIF_SHIM_LIB) $(EMU_LIB)
 
-$(EMU_LIB): $(EMU_SRCS) $(wildcard tests/emu/*.h) $(wildcard tests/emu/*.cuh) $(HDRS)
+$(EMU_LIB): $(EMU_SRCS) $(wildcard tests/emu/*.h) $(wildcard tests/emu/*.cuh) $(wildcard tests/emu/nvcomp/device/detail/*.cuh) $(HDRS)
 	g++ -std=c++17 -O2 -g -fPIC -shared -Wall -Wno-unknown-pragmas -Wno-unused-function \
 	    -Itests/emu -I$(SRC_DIR) -Iinclude -I/usr/local/cuda/include $(EMU_SRCS) -o $@
 
@@ -63,6 +65,11 @@ $(CASCADED_DEVICE_LIB): tests/cpp/cascaded_device_kernels.cu $(HDRS)
 	@mkdir -p build/tests
 	$(NVCC) $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -shared -Xptxas -v $< -o $@ \
 	    2> build/tests/libcascaded_device.ptxas.log || (cat build/tests/libcascaded_device.ptxas.log; exit 1)
+
+$(LZ_DEVICE_LIB): tests/cpp/lz_device_kernels.cu $(HDRS)
+	@mkdir -p build/tests
+	$(NVCC) $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -shared -Xptxas -v $< -o $@ \
+	    2> build/tests/liblz_device.ptxas.log || (cat build/tests/liblz_device.ptxas.log; exit 1)
 
 $(HLIF_SHIM_LIB): tests/cpp/hlif_shim.cu $(LIB) $(HDRS)
 	@mkdir -p build/tests

@@ -12,6 +12,7 @@
 // matches are 16-byte vector copies: common.cuh warp_copy / warp_match_copy).
 #include "common.cuh"
 #include "lz77_compress.cuh"
+#include "nvcomp/device/detail/lz4_encode.cuh"
 #include "lz4_decode.cuh"
 #include "lz_sched.cuh"
 #include "nvcomp/lz4.h"
@@ -133,36 +134,9 @@ lz4_decompress_v2_kernel(const void* const* __restrict__ comp_ptrs,
 // ---------------------------------------------------------------------------
 // Compression
 // ---------------------------------------------------------------------------
-struct Lz4Emitter {
-  uint8_t* out;
-  uint32_t op;
-
-  __device__ __forceinline__ void ext(uint32_t rem, int lane) {   // rem = len - 15
-    const uint32_t nb = rem / 255u + 1u;
-    for (uint32_t i = lane; i < nb; i += kWarp)
-      out[op + i] = (i + 1 < nb) ? (uint8_t)255 : (uint8_t)(rem - 255u * (nb - 1));
-    op += nb;
-  }
-  __device__ __forceinline__ void sequence(const uint8_t* lit, uint32_t ll, uint32_t off,
-                                           uint32_t ml, int lane) {
-    const uint32_t mlc = ml - 4;
-    if (lane == 0) out[op] = (uint8_t)((min(ll, 15u) << 4) | min(mlc, 15u));
-    op += 1;
-    if (ll >= 15) ext(ll - 15, lane);
-    if (ll) warp_copy<true>(out + op, lit, ll, lane);
-    op += ll;
-    if (lane == 0) { out[op] = (uint8_t)(off & 255u); out[op + 1] = (uint8_t)(off >> 8); }
-    op += 2;
-    if (mlc >= 15) ext(mlc - 15, lane);
-  }
-  __device__ __forceinline__ void finish(const uint8_t* lit, uint32_t ll, int lane) {
-    if (lane == 0) out[op] = (uint8_t)(min(ll, 15u) << 4);
-    op += 1;
-    if (ll >= 15) ext(ll - 15, lane);
-    if (ll) warp_copy<true>(out + op, lit, ll, lane);
-    op += ll;
-  }
-};
+// the LZ4 emitter of the matcher, shared with the device API (nvcomp/device/detail/lz4_encode.cuh)
+using nvcomp::device::lz::detail::Lz4Emitter;
+using nvcomp::device::lz::detail::lz4_step_for;
 
 constexpr int kCompWarpsPerCta = 4;
 
@@ -186,16 +160,6 @@ lz4_compress_kernel(const void* const* __restrict__ in_ptrs, const size_t* __res
     lz77_compress_chunk(in, n, em, table, step, 5u, 12u, lane);
     if (lane == 0) out_bytes[c] = em.op;
     __syncwarp();
-  }
-}
-
-inline uint32_t lz4_step_for(nvcompType_t t, bool* ok) {
-  *ok = true;
-  switch (t) {
-    case NVCOMP_TYPE_CHAR: case NVCOMP_TYPE_UCHAR: case NVCOMP_TYPE_BITS: return 1;
-    case NVCOMP_TYPE_SHORT: case NVCOMP_TYPE_USHORT: return 2;
-    case NVCOMP_TYPE_INT: case NVCOMP_TYPE_UINT: return 4;
-    default: *ok = false; return 1;
   }
 }
 
