@@ -22,6 +22,12 @@ BITCOMP_DEVICE_LIB := build/tests/libbitcomp_device.so
 CASCADED_DEVICE_LIB := build/tests/libcascaded_device.so
 # kernels over the warp-level LZ4 and Snappy device APIs (include/nvcomp/device/{lz4,snappy}.cuh), loaded the same way
 LZ_DEVICE_LIB := build/tests/liblz_device.so
+# kernels over the warp-level Deflate, Gzip and Zstd device APIs (include/nvcomp/device/{deflate,gzip,zstd}.cuh), loaded
+# the same way
+DZ_DEVICE_LIB := build/tests/libdeflate_zstd_device.so
+# one library linked from two translation units that include all eight device headers, plain and with -rdc=true: the
+# headers must not define functions with external, non-inline linkage (tests/cpp/device_headers_link.cu)
+LINK_LIBS := build/tests/libdevice_headers_link.so build/tests/libdevice_headers_link_rdc.so
 # extern "C" dispatch onto the C++ managers (nvcomp::*Manager, create_manager), loaded the same way
 HLIF_SHIM_LIB := build/tests/libhlif_shim.so
 
@@ -30,7 +36,7 @@ EMU_LIB  := tests/emu/libemu_lz.so
 EMU_SRCS := tests/emu/emu_cuda.cpp tests/emu/emu_lz.cpp tests/emu/emu_inflate.cpp tests/emu/emu_deflate.cpp \
             tests/emu/emu_zstd.cpp
 
-all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(ANS_DEVICE_LIB) $(BITCOMP_DEVICE_LIB) $(CASCADED_DEVICE_LIB) $(LZ_DEVICE_LIB) $(HLIF_SHIM_LIB) $(EMU_LIB)
+all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(ANS_DEVICE_LIB) $(BITCOMP_DEVICE_LIB) $(CASCADED_DEVICE_LIB) $(LZ_DEVICE_LIB) $(DZ_DEVICE_LIB) $(LINK_LIBS) $(HLIF_SHIM_LIB) $(EMU_LIB)
 
 $(EMU_LIB): $(EMU_SRCS) $(wildcard tests/emu/*.h) $(wildcard tests/emu/*.cuh) $(wildcard tests/emu/nvcomp/device/detail/*.cuh) $(HDRS)
 	g++ -std=c++17 -O2 -g -fPIC -shared -Wall -Wno-unknown-pragmas -Wno-unused-function \
@@ -70,6 +76,25 @@ $(LZ_DEVICE_LIB): tests/cpp/lz_device_kernels.cu $(HDRS)
 	@mkdir -p build/tests
 	$(NVCC) $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -shared -Xptxas -v $< -o $@ \
 	    2> build/tests/liblz_device.ptxas.log || (cat build/tests/liblz_device.ptxas.log; exit 1)
+
+$(DZ_DEVICE_LIB): tests/cpp/deflate_zstd_device_kernels.cu $(HDRS)
+	@mkdir -p build/tests
+	$(NVCC) $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -shared -Xptxas -v $< -o $@ \
+	    2> build/tests/libdeflate_zstd_device.ptxas.log || (cat build/tests/libdeflate_zstd_device.ptxas.log; exit 1)
+
+build/tests/link_tu%.o: tests/cpp/device_headers_link.cu $(HDRS)
+	@mkdir -p build/tests
+	$(NVCC) $(ARCH) -O3 -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -DLINK_TU=$* -c $< -o $@
+
+build/tests/link_rdc_tu%.o: tests/cpp/device_headers_link.cu $(HDRS)
+	@mkdir -p build/tests
+	$(NVCC) $(ARCH) -O3 -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -rdc=true -DLINK_TU=$* -c $< -o $@
+
+build/tests/libdevice_headers_link.so: build/tests/link_tu1.o build/tests/link_tu2.o
+	$(NVCC) $(ARCH) -shared $^ -o $@
+
+build/tests/libdevice_headers_link_rdc.so: build/tests/link_rdc_tu1.o build/tests/link_rdc_tu2.o
+	$(NVCC) $(ARCH) -rdc=true -shared $^ -o $@
 
 $(HLIF_SHIM_LIB): tests/cpp/hlif_shim.cu $(LIB) $(HDRS)
 	@mkdir -p build/tests
