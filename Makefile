@@ -36,7 +36,7 @@ HLIF_SHIM_LIB := build/tests/libhlif_shim.so
 # host warp emulator (test infrastructure): the warp-level decode headers compiled with g++, PTX shadowed
 EMU_LIB  := tests/emu/libemu_lz.so
 EMU_SRCS := tests/emu/emu_cuda.cpp tests/emu/emu_lz.cpp tests/emu/emu_inflate.cpp tests/emu/emu_deflate.cpp \
-            tests/emu/emu_zstd.cpp tests/emu/emu_zstd_encode.cpp
+            tests/emu/emu_zstd.cpp tests/emu/emu_zstd_encode.cpp tests/emu/emu_lz_encode.cpp
 
 all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(ANS_DEVICE_LIB) $(BITCOMP_DEVICE_LIB) $(CASCADED_DEVICE_LIB) $(LZ_DEVICE_LIB) $(DZ_DEVICE_LIB) $(ZC_DEVICE_LIB) $(LINK_LIBS) $(HLIF_SHIM_LIB) $(EMU_LIB)
 

@@ -66,7 +66,6 @@ static_assert(kPmWords * 4 <= kHashBytesPerWarp, "package-merge workspace fits i
 template <int kAlgo> struct DeflateAlgo;
 template <> struct DeflateAlgo<0> : LzParams {          // high throughput: the greedy matcher
   static constexpr uint32_t kMaxDist = 32768u, kMaxLen = 258u;
-  static constexpr bool kDetInsert = true;
   static constexpr bool kParse = true;
 };
 template <> struct DeflateAlgo<1> : DeflateAlgo<0> {    // high compression: bigger table, lazy step

@@ -43,6 +43,15 @@ struct Lz4Emitter {
   }
 };
 
+// The matcher's parse of one LZ4 block of the n bytes at `in`, into em (an Lz4Emitter writes the block).  LZ4's
+// end-of-block rules: the last 5 bytes are literals, and the last match starts at least 12 bytes before the end
+// (reference CHANGELOG.md:195).  step: the data_type's candidate stride.
+template <class Emitter>
+__device__ __forceinline__ void lz4_compress_chunk(const uint8_t* __restrict__ in, uint32_t n, Emitter& em,
+                                                   uint16_t* table, uint32_t step, int lane) {
+  lz77_compress_chunk(in, n, em, table, step, 5u, 12u, lane);
+}
+
 // Candidate stride (bytes) of the matcher for an LZ4 data_type; *ok = false for a type the LZ4 calls reject.
 __host__ __device__ inline uint32_t lz4_step_for(nvcompType_t t, bool* ok) {
   *ok = true;

@@ -11,11 +11,14 @@
 // correct and reasonably parallel, not ratio-optimal: greedy parse, no
 // back-extension.  Matches are >= 4 bytes (the hash covers 4 bytes).
 //
+// Hash inserts are deterministic: when several lanes of a round insert into one bucket, the highest lane's position
+// is the one kept.  A same-address shared store from several lanes has no defined winner on the GPU, so without
+// this a stream would depend on the hardware as well as on its input; every encoder's stream is pinned byte for
+// byte to the host emulator.
+//
 // Compile-time parameters (LzParams): LZ4 and Snappy use the defaults.  Deflate sets a 32 768-byte window, a
-// 258-byte match limit (cooperative extension stops there), a deterministic hash insert (when several lanes of a
-// round insert into one bucket, the highest lane's position is the one kept: a same-address shared store from
-// several lanes has no defined winner on the GPU, and the Deflate stream is pinned byte for byte to the host
-// emulator), and, for its high-compression mode, a 2^15-entry table and one-position lazy evaluation.
+// 258-byte match limit (cooperative extension stops there) and, for its high-compression mode, a 2^15-entry table
+// and one-position lazy evaluation.
 #pragma once
 
 #include "nvcomp/device/detail/lz_common.cuh"
@@ -38,7 +41,6 @@ struct LzParams {
   static constexpr int kHashLog = detail::kHashLog;
   static constexpr uint32_t kMaxDist = 65535u;
   static constexpr uint32_t kMaxLen = 0;        // 0: no limit
-  static constexpr bool kDetInsert = false;
   // after a match starting at p is found, if position p + 1 (the next lane, stride 1 only) has a longer verified
   // match at a distance no larger, p becomes a literal and that match is taken instead (one step, not chained).
   // Without the distance condition a Deflate stream of float columns grows: the longer match is often far back,
@@ -135,8 +137,7 @@ __device__ __forceinline__ void lz77_compress_chunk(
     }
     unsigned m = __ballot_sync(kFull, is_match);
     if (m == 0) {
-      if constexpr (P::kDetInsert) det_insert(table, h, p, valid, lane);
-      else if (valid) table[h] = (uint16_t)p;
+      det_insert(table, h, p, valid, lane);
       __syncwarp();
       pos += 32u * step * accel;
       if (misses < 64) ++misses;
@@ -166,9 +167,6 @@ __device__ __forceinline__ void lz77_compress_chunk(
       }
       const int first = first0 + lazy;
       if (step > 1) len &= ~(step - 1);   // keep candidate positions element-aligned
-      if constexpr (!P::kDetInsert) {
-        if (valid && lane > prev_first && lane <= first) table[h] = (uint16_t)p;
-      }
       prev_first = first;
       if (len < 4) {                       // too short after limits: not a match after all
         m &= ~(1u << first);
@@ -183,7 +181,7 @@ __device__ __forceinline__ void lz77_compress_chunk(
       m &= ~((1u << skip) - 1u);
     }
     // the table is read only at the start of a round, so the inserts can wait for its end
-    if constexpr (P::kDetInsert) det_insert(table, h, p, valid && lane <= prev_first, lane);
+    det_insert(table, h, p, valid && lane <= prev_first, lane);
     __syncwarp();
     pos = (new_pos > pos) ? new_pos : pos + 32u * stride;
   }

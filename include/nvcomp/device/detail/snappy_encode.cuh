@@ -76,6 +76,15 @@ struct SnappyEmitter {
   }
 };
 
+// The matcher's parse of the n bytes at `in` after the preamble, into em (a SnappyEmitter, after em.begin(n), writes
+// the stream).  Snappy has no end-of-block rules; a match starts at least 4 bytes before the end, which keeps the
+// 4-byte probe in bounds.
+template <class Emitter>
+__device__ __forceinline__ void snappy_compress_chunk(const uint8_t* __restrict__ in, uint32_t n, Emitter& em,
+                                                      uint16_t* table, int lane) {
+  lz77_compress_chunk(in, n, em, table, 1u, 0u, 4u, lane);
+}
+
 }  // namespace detail
 }  // namespace lz
 }  // namespace device

@@ -15,7 +15,7 @@
 //     the literals and records of a block must fit in the region next to the hash table; libzstd level 1 loses
 //     0.2-3 % of its ratio on the datagen tables when it cuts 64 KB chunks into independent 16 KB frames, and 21 % on
 //     run-length int32, whose matches span blocks -- here blocks share history, so the loss is lower.)
-//   * Parse: lz77_compress_chunk with ZstdLzParams -- greedy, deterministic hash inserts, distance <= 65 535,
+//   * Parse: lz77_compress_chunk with the default LzParams -- greedy, deterministic hash inserts, distance <= 65 535,
 //     matches >= 4 bytes, as the matcher finds them; matches may reach into earlier blocks.  A match that crosses a
 //     block end is split there; a piece shorter than 4 bytes becomes literals.
 //   * Repeat offsets (RFC 8878 3.1.2.5): the history starts at (1, 4, 8) per frame and is updated by every
@@ -61,11 +61,6 @@ using deflate::detail::DeflateBits;
 constexpr uint32_t kZstdBlockBytes = 16384;
 constexpr uint32_t kZstdMaxCompressChunk = 65536;
 constexpr uint32_t kZeHufLimit = 11;
-
-struct ZstdLzParams : lz::detail::LzParams {
-  static constexpr uint32_t kMaxDist = 65535u;
-  static constexpr bool kDetInsert = true;
-};
 
 // Per-warp region (byte offsets).  ws is the package-merge workspace while the Huffman code is built, then the FSE
 // state tables, one decode table and the decoder's table-builder scratch.
@@ -719,7 +714,7 @@ __device__ __forceinline__ uint32_t zstd_compress_chunk(const uint8_t* __restric
   uint32_t* h = e.w.hist();
   for (int i = lane; i < 256; i += kWarp) h[i] = 0;
   __syncwarp();
-  lz77_compress_chunk<ZstdEnc, ZstdLzParams>(in, n, e, e.w.table(), 1u, 0u, 4u, lane);
+  lz77_compress_chunk(in, n, e, e.w.table(), 1u, 0u, 4u, lane);
   __syncwarp();
   return e.o;
 }

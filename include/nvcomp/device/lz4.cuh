@@ -112,9 +112,7 @@ __device__ inline nvcompStatus_t compress_warp(const void* in, size_t n_bytes, v
     return st;
   }
   Lz4Emitter em{(uint8_t*)out, 0};
-  // LZ4 end-of-block rules, as lz4_compress_kernel: the last 5 bytes are literals, the last match starts at least
-  // 12 bytes before the end
-  lz77_compress_chunk((const uint8_t*)in, (uint32_t)n_bytes, em, (uint16_t*)smem, step, 5u, 12u, lane);
+  lz4_compress_chunk((const uint8_t*)in, (uint32_t)n_bytes, em, (uint16_t*)smem, step, lane);
   if (lane == 0 && comp_bytes) *comp_bytes = em.op;
   __syncwarp();
   return nvcompSuccess;

@@ -99,8 +99,7 @@ __device__ inline nvcompStatus_t compress_warp(const void* in, size_t n_bytes, v
   }
   SnappyEmitter em{(uint8_t*)out, 0};
   em.begin((uint32_t)n_bytes, lane);
-  // as snappy_compress_kernel: no end-of-block restrictions; 4 keeps the 4-byte probe in bounds
-  lz77_compress_chunk((const uint8_t*)in, (uint32_t)n_bytes, em, (uint16_t*)smem, 1u, 0u, 4u, lane);
+  snappy_compress_chunk((const uint8_t*)in, (uint32_t)n_bytes, em, (uint16_t*)smem, lane);
   if (lane == 0 && comp_bytes) *comp_bytes = em.op;
   __syncwarp();
   return nvcompSuccess;

@@ -136,13 +136,14 @@ lz4_decompress_v2_kernel(const void* const* __restrict__ comp_ptrs,
 // ---------------------------------------------------------------------------
 // the LZ4 emitter of the matcher, shared with the device API (nvcomp/device/detail/lz4_encode.cuh)
 using nvcomp::device::lz::detail::Lz4Emitter;
+using nvcomp::device::lz::detail::lz4_compress_chunk;
 using nvcomp::device::lz::detail::lz4_step_for;
 
 constexpr int kCompWarpsPerCta = 4;
 
 __global__ void __launch_bounds__(kCompWarpsPerCta * 32)
 lz4_compress_kernel(const void* const* __restrict__ in_ptrs, const size_t* __restrict__ in_bytes,
-                    size_t batch, void* const* __restrict__ out_ptrs, size_t* out_bytes,
+                    size_t max_chunk, size_t batch, void* const* __restrict__ out_ptrs, size_t* out_bytes,
                     uint32_t step, unsigned long long* ticket) {
   extern __shared__ __align__(16) uint8_t smem[];
   const int lane = lane_id();
@@ -153,11 +154,10 @@ lz4_compress_kernel(const void* const* __restrict__ in_ptrs, const size_t* __res
   WarpTicket sched(ticket, warp_global, warps_total);
   for (size_t c = sched.next(lane); c < batch; c = sched.next(lane)) {
     const uint8_t* in = (const uint8_t*)in_ptrs[c];
-    const uint32_t n = (uint32_t)in_bytes[c];
+    // a chunk over max_chunk gets size 0 and nothing else: its stream could outgrow the output slot the caller
+    // sized with GetMaxOutputChunkSize(max_chunk)
     Lz4Emitter em{(uint8_t*)out_ptrs[c], 0};
-    // LZ4 end-of-block rules: last 5 bytes are literals, the last match starts
-    // at least 12 bytes before the end (reference CHANGELOG.md:195).
-    lz77_compress_chunk(in, n, em, table, step, 5u, 12u, lane);
+    if (in_bytes[c] <= max_chunk) lz4_compress_chunk(in, (uint32_t)in_bytes[c], em, table, step, lane);
     if (lane == 0) out_bytes[c] = em.op;
     __syncwarp();
   }
@@ -212,7 +212,7 @@ nvcompStatus_t nvcompBatchedLZ4CompressAsync(
   B200_CUDA_TRY(ensure_dynamic_smem(lz4_compress_kernel, (int)smem, smem_set));
   const int grid = persistent_grid(6, batch, kCompWarpsPerCta);
   lz4_compress_kernel<<<grid, kCompWarpsPerCta * 32, smem, stream>>>(
-      in_ptrs, in_bytes, batch, out_ptrs, out_bytes, step, ticket);
+      in_ptrs, in_bytes, max_chunk, batch, out_ptrs, out_bytes, step, ticket);
   B200_CUDA_TRY(cudaGetLastError());
   return nvcompSuccess;
 }

@@ -129,12 +129,13 @@ __global__ void snappy_size_kernel(const void* const* __restrict__ comp_ptrs,
 // ---------------------------------------------------------------------------
 // the Snappy emitter of the matcher, shared with the device API (nvcomp/device/detail/snappy_encode.cuh)
 using nvcomp::device::lz::detail::SnappyEmitter;
+using nvcomp::device::lz::detail::snappy_compress_chunk;
 
 constexpr int kSnappyCompWarps = 4;
 
 __global__ void __launch_bounds__(kSnappyCompWarps * 32)
 snappy_compress_kernel(const void* const* __restrict__ in_ptrs, const size_t* __restrict__ in_bytes,
-                       size_t batch, void* const* __restrict__ out_ptrs, size_t* out_bytes,
+                       size_t max_chunk, size_t batch, void* const* __restrict__ out_ptrs, size_t* out_bytes,
                        unsigned long long* ticket) {
   extern __shared__ __align__(16) uint8_t smem[];
   const int lane = lane_id();
@@ -145,11 +146,13 @@ snappy_compress_kernel(const void* const* __restrict__ in_ptrs, const size_t* __
   WarpTicket sched(ticket, warp_global, warps_total);
   for (size_t c = sched.next(lane); c < batch; c = sched.next(lane)) {
     const uint8_t* in = (const uint8_t*)in_ptrs[c];
-    const uint32_t n = (uint32_t)in_bytes[c];
+    // a chunk over max_chunk gets size 0 and nothing else: its stream could outgrow the output slot the caller
+    // sized with GetMaxOutputChunkSize(max_chunk)
     SnappyEmitter em{(uint8_t*)out_ptrs[c], 0};
-    em.begin(n, lane);
-    // Snappy has no end-of-block restrictions; 4 keeps the 4-byte probe in bounds.
-    lz77_compress_chunk(in, n, em, table, 1u, 0u, 4u, lane);
+    if (in_bytes[c] <= max_chunk) {
+      em.begin((uint32_t)in_bytes[c], lane);
+      snappy_compress_chunk(in, (uint32_t)in_bytes[c], em, table, lane);
+    }
     if (lane == 0) out_bytes[c] = em.op;
     __syncwarp();
   }
@@ -200,7 +203,7 @@ nvcompStatus_t nvcompBatchedSnappyCompressAsync(
   B200_CUDA_TRY(ensure_dynamic_smem(snappy_compress_kernel, (int)smem, smem_set));
   const int grid = persistent_grid(6, batch, kSnappyCompWarps);
   snappy_compress_kernel<<<grid, kSnappyCompWarps * 32, smem, stream>>>(
-      in_ptrs, in_bytes, batch, out_ptrs, out_bytes, ticket);
+      in_ptrs, in_bytes, max_chunk, batch, out_ptrs, out_bytes, ticket);
   B200_CUDA_TRY(cudaGetLastError());
   return nvcompSuccess;
 }
