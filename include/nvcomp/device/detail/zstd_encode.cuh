@@ -35,7 +35,9 @@
 //     distinct code) or FSE_Compressed, whichever has the lowest cost: sum over codes of count * (log - log2(p))
 //     bits, with log2 taken as highbit + linear mantissa in 1/256 bit, plus 8 bits for RLE or 8 bits per header
 //     byte for FSE; ties Predefined, then RLE.  Repeat_Mode is not used.  FSE counts: accuracy log libzstd's
-//     FSE_optimalTableLog(max, nseq, max code) with max 9 (LL, ML) or 8 (OF); each used code gets
+//     FSE_optimalTableLog(max, nseq, max code) with max 9 (LL, ML) or 8 (OF) for nseq >= 5, and 5 below (where
+//     libzstd's unsigned highbit(nseq - 1) - 2 wraps and it would keep max: a block of 4 sequences with OF codes
+//     0, 0, 0, 1 takes FSE at log 5 and would take Predefined at log 8); each used code gets
 //     max(1, count * 2^log / nseq), and the difference to 2^log goes to the most frequent code (lowest code on
 //     ties) or, when negative, is taken from the largest counts down to 1.  The counts are written as RFC 8878 4.1.1
 //     (libzstd's FSE_writeNCount).  The bitstream follows the RFC's order; each state starts on the first cell (in
@@ -123,7 +125,7 @@ __device__ __forceinline__ uint32_t ze_cost(uint32_t c, uint32_t log) {
   return (log << 8) - ((hb << 8) + (((c << 8) >> hb) - 256u));
 }
 
-// libzstd FSE_optimalTableLog
+// libzstd FSE_optimalTableLog for n >= 5; 5 for n < 5 (the file header says why)
 __device__ __forceinline__ uint32_t ze_table_log(uint32_t max_log, uint32_t n, uint32_t max_sym) {
   const uint32_t src_bits = n > 1u ? zs_highbit(n - 1u) : 0u;
   uint32_t log = max_log;

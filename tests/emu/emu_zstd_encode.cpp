@@ -56,11 +56,45 @@ struct Guarded {
   ~Guarded() { munmap(map, map_bytes); }
 };
 
+// Records the parse: (literal run, offset, length) per sequence, (trailing literals, 0, 0) at the end.
+struct TokenRec {
+  uint32_t* t;
+  uint32_t cap, n;
+  void put(uint32_t a, uint32_t b, uint32_t c, int lane) {
+    if (lane == 0 && n + 3 <= cap) { t[n] = a; t[n + 1] = b; t[n + 2] = c; }
+    n += 3;
+  }
+  void sequence(const uint8_t*, uint32_t ll, uint32_t off, uint32_t ml, int lane) { put(ll, off, ml, lane); }
+  void finish(const uint8_t*, uint32_t ll, int lane) { put(ll, 0, 0, lane); }
+};
+
 }  // namespace
 
 extern "C" {
 size_t emu_zstd_enc_bound(size_t n) { return zd::zstd_enc_bound((uint32_t)n); }
 size_t emu_zstd_enc_smem(void) { return zd::kZstdEncWarpSmem; }
+
+// The matcher's parse of n <= 64 KB bytes with the encoder's own arguments (zstd_compress_chunk), before it is cut
+// into blocks: (literal run, offset, length) triples into t (cap words; a trailing (literals, 0, 0)).  Returns the
+// number of words, or -2 on an emulator fault.
+long emu_zstd_parse(const uint8_t* src, size_t n, uint32_t* t, size_t cap, char* msg, size_t msg_bytes) {
+  Guarded gin(n, 0);
+  if (n) memcpy(gin.p, src, n);
+  emu::Warp w;
+  emu::add_region(w, gin.p, n, false);
+  uint32_t words = 0;
+  emu::run_warp(w, zd::kZstdEncWarpSmem, [&](int lane) {
+    TokenRec rec{t, (uint32_t)cap, 0};
+    zd::lz77_compress_chunk(gin.p, (uint32_t)n, rec, (uint16_t*)(emu::g_warp->smem + zd::kZeHashOff), 1u, 0u, 4u,
+                            lane);
+    if (lane == 0) words = rec.n;
+  });
+  if (w.failed) {
+    if (msg) snprintf(msg, msg_bytes, "%s", w.fail_msg);
+    return -2;
+  }
+  return (long)words;
+}
 
 // Compress n <= 64 KB bytes (input at misalignment in_mis, output at out_mis) into dst, which has room for the
 // bound.  Returns the frame length, or -2 on an emulator fault or a write past the frame (msg says why).

@@ -169,16 +169,19 @@ def _roundtrip(lib, zs, chunks, kind):
     frames = out.to_host()
     for i in np.random.default_rng(1).choice(len(chunks), 40, replace=False):
         assert zs.expect(frames[i], 65536) == ("ok", chunks[i]), (kind, i)
-    return sum(len(f) for f in frames)
+    return frames
 
 
 @pytest.mark.parametrize("kind", ["tabular_f32", "runlength_i32"])
-def test_roundtrip_10000_chunks(lib, zs, kind):
+def test_roundtrip_10000_chunks(lib, zs, emu, kind):
     raw = (datagen.tabular_f32(10000) if kind == "tabular_f32" else datagen.runlength_i32(10000)).tobytes()
     chunks = [raw[i:i + 65536] for i in range(0, len(raw), 65536)]
     assert len(chunks) == 10000
-    comp = _roundtrip(lib, zs, chunks, kind)
-    assert comp < len(raw) / (2.3 if kind == "tabular_f32" else 60)
+    frames = _roundtrip(lib, zs, chunks, kind)
+    assert sum(map(len, frames)) < len(raw) / (2.3 if kind == "tabular_f32" else 60)
+    # the frames of 64 seeded chunks are the emulator's byte for byte
+    for i in np.random.default_rng(2).choice(len(chunks), 64, replace=False):
+        assert frames[i] == emu.compress(chunks[i]), (kind, i)
 
 
 def test_mixed_cta(lib, emu):

@@ -23,9 +23,22 @@ class EmuZstdEncoder:
         self.lib.emu_zstd_enc_bound.restype = C.c_size_t
         self.lib.emu_zstd_enc_bound.argtypes = [C.c_size_t]
         self.lib.emu_zstd_enc_smem.restype = C.c_size_t
+        self.lib.emu_zstd_parse.restype = C.c_long
+        self.lib.emu_zstd_parse.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_char_p, C.c_size_t]
 
     def bound(self, n: int) -> int:
         return self.lib.emu_zstd_enc_bound(n)
+
+    def parse(self, data: bytes):
+        """The matcher's parse with the encoder's arguments, before block cutting:
+        [(literal run, offset, length), ..., (trailing literals, 0, 0)]."""
+        cap = 3 * (len(data) // 4 + 2)
+        t = (C.c_uint32 * cap)()
+        msg = C.create_string_buffer(256)
+        r = self.lib.emu_zstd_parse(data, len(data), t, cap, msg, 256)
+        assert r != FAULT, f"emulator fault: {msg.value.decode()}"
+        assert 0 < r <= cap, r
+        return [tuple(t[i:i + 3]) for i in range(0, r, 3)]
 
     def compress(self, data: bytes, in_mis: int = 0, out_mis: int = 0) -> bytes:
         """One frame; the emulator also checks that nothing past the frame was written."""
@@ -48,6 +61,88 @@ def fibonacci_bytes(n=65536, seed=5):
     data = np.repeat(np.arange(22, dtype=np.uint8) * 11, counts)
     np.random.default_rng(seed).shuffle(data)
     return data.tobytes()
+
+
+def literal_run(m, seed, n=8192):
+    """m random bytes, then their last 64 bytes repeated up to n: one literal run, then one long match."""
+    y = np.random.default_rng(seed).integers(0, 256, m, dtype=np.uint8).tobytes()
+    return (y + y[-64:] * (n // 64 + 1))[:n]
+
+
+def short_runs(c, a, last, seed):
+    """64 random bytes, then c pieces of `a` random literals (`last` in the final piece) and an 8-byte copy from the
+    first 64 bytes: about one sequence per piece."""
+    rng = np.random.default_rng(seed)
+    r = rng.integers(0, 256, 64, dtype=np.uint8)
+    parts = [r.tobytes()]
+    for i in range(c):
+        j = int(rng.integers(0, 56))
+        parts.append(rng.integers(0, 256, a if i < c - 1 else last, dtype=np.uint8).tobytes() + r[j:j + 8].tobytes())
+    return b"".join(parts)
+
+
+def copy_pieces(c, seed):
+    """256 random bytes, then c pieces of one random literal and an 8-byte copy from them."""
+    rng = np.random.default_rng(seed)
+    r = rng.integers(0, 256, 256, dtype=np.uint8)
+    parts = [r.tobytes()]
+    for _ in range(c):
+        j = int(rng.integers(0, 240))
+        parts.append(bytes([int(rng.integers(0, 256))]) + r[j:j + 8].tobytes())
+    parts.append(rng.integers(0, 256, 16, dtype=np.uint8).tobytes())
+    return b"".join(parts)
+
+
+def tail_repeat(n, k, seed):
+    """n random bytes whose last k repeat the first k."""
+    y = np.random.default_rng(seed).integers(0, 256, n, dtype=np.uint8).tobytes()
+    return y[:n - k] + y[:k]
+
+
+def skewed_literals(seed, n=400):
+    """n bytes from a geometric distribution over a random subset of the symbols below 128."""
+    rng = np.random.default_rng(seed)
+    nsym = int(rng.integers(3, 40))
+    syms = rng.choice(int(rng.integers(nsym, 128)), nsym, replace=False)
+    p = rng.geometric(float(rng.uniform(0.05, 0.5)), n) % nsym
+    return syms[p].astype(np.uint8).tobytes()
+
+
+def one_literal_block():
+    """Block 1: 1 000 random bytes, then "ab" repeated; block 2: the byte that ends that match, then the 1 000 bytes
+    again: its literals section holds exactly one literal."""
+    r = np.random.default_rng(5).integers(0, 256, 1000, dtype=np.uint8).tobytes()
+    return r + (b"ab" * 9000)[:16384 - 1000] + b"a" + r
+
+
+def boundary_inputs():
+    """Inputs whose first block sits on one side of a stream-rule boundary (the seeds and sizes were searched for
+    with the matcher and tests/zstd_encode_model.py; tests/test_zstd_encode_model.py asserts each boundary is hit)."""
+    rng = np.random.default_rng(1)
+    raw_first = bytearray(rng.integers(0, 256, 16384, dtype=np.uint8).tobytes())
+    raw_first[9000:9005] = raw_first[100:105]          # a 5-byte match that does not pay for itself
+    raw_then_repeat = (bytes(raw_first) + rng.integers(0, 256, 40, dtype=np.uint8).tobytes() + bytes([7]) * 200 +
+                       rng.integers(0, 256, 40, dtype=np.uint8).tobytes())
+    return {
+        "raw_lits31": literal_run(31, 31),                        # Raw literals, 1-byte header
+        "raw_lits32": literal_run(32, 32),                        # 2-byte header
+        "raw_lits4095": short_runs(160, 25, 14, 4095),            # 2-byte header
+        "raw_lits4096": short_runs(158, 25, 46, 4096),            # 3-byte header
+        "huf_lits255": (np.random.default_rng(1000).integers(0, 32, 255, dtype=np.uint8).tobytes() * 9)[:2048],
+        "huf_lits256": (np.random.default_rng(1000).integers(0, 32, 256, dtype=np.uint8).tobytes() * 8)[:2048],
+        "huf_lits16384": np.random.default_rng(0).integers(0, 128, 16384, dtype=np.uint8).tobytes(),   # no match
+        "nseq127": copy_pieces(114, 7),
+        "nseq128": copy_pieces(115, 7),
+        "body_block_minus1": tail_repeat(600, 10, 0),             # Compressed body of 599 bytes
+        "body_equals_block": tail_repeat(600, 8, 162),            # Compressed body of 600 bytes: Raw
+        "raw_then_repeat": raw_then_repeat,
+        "one_literal_block": one_literal_block(),                 # Raw and RLE literals of the same size
+        "weights_tie": skewed_literals(242),                      # direct and FSE weights of the same size
+        "table_cost_tie": copy_pieces(6, 1),                      # ML: Predefined and FSE of the same cost
+        # 4 sequences, OF codes 0, 0, 0, 1: an FSE table at accuracy log 5
+        "fse_four_sequences": b"abx" + b"x" * 20 + b"cdy" + b"y" * 20 + b"efz" + b"z" * 20 + b"gh" + b"klmn" * 6 +
+                              b"pqrstuvw",
+    }
 
 
 def edge_inputs():
@@ -84,6 +179,7 @@ def edge_inputs():
         "distance65532": far + far[:4],
         "match_across_block": half + half + half[:5000],
         "text_17000": text[:17000],
+        **boundary_inputs(),
     }
 
 
