@@ -27,6 +27,8 @@ LZ_DEVICE_LIB := build/tests/liblz_device.so
 DZ_DEVICE_LIB := build/tests/libdeflate_zstd_device.so
 # kernels over zstd::compress_warp (include/nvcomp/device/zstd.cuh), loaded the same way
 ZC_DEVICE_LIB := build/tests/libzstd_compress_device.so
+# kernels over the warp-level LZ4 frame device API (include/nvcomp/device/lz4frame.cuh), loaded the same way
+LZ4F_DEVICE_LIB := build/tests/liblz4frame_device.so build/tests/liblz4frame_device_rdc.so
 # one library linked from two translation units that include all eight device headers, plain and with -rdc=true: the
 # headers must not define functions with external, non-inline linkage (tests/cpp/device_headers_link.cu)
 LINK_LIBS := build/tests/libdevice_headers_link.so build/tests/libdevice_headers_link_rdc.so
@@ -36,9 +38,10 @@ HLIF_SHIM_LIB := build/tests/libhlif_shim.so
 # host warp emulator (test infrastructure): the warp-level decode headers compiled with g++, PTX shadowed
 EMU_LIB  := tests/emu/libemu_lz.so
 EMU_SRCS := tests/emu/emu_cuda.cpp tests/emu/emu_lz.cpp tests/emu/emu_inflate.cpp tests/emu/emu_deflate.cpp \
-            tests/emu/emu_zstd.cpp tests/emu/emu_zstd_encode.cpp tests/emu/emu_lz_encode.cpp
+            tests/emu/emu_zstd.cpp tests/emu/emu_zstd_encode.cpp tests/emu/emu_lz_encode.cpp \
+            tests/emu/emu_lz4frame.cpp
 
-all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(ANS_DEVICE_LIB) $(BITCOMP_DEVICE_LIB) $(CASCADED_DEVICE_LIB) $(LZ_DEVICE_LIB) $(DZ_DEVICE_LIB) $(ZC_DEVICE_LIB) $(LINK_LIBS) $(HLIF_SHIM_LIB) $(EMU_LIB)
+all: $(LIB) $(ORACLE_LIB) $(TESTS_BIN) $(ANS_DEVICE_LIB) $(BITCOMP_DEVICE_LIB) $(CASCADED_DEVICE_LIB) $(LZ_DEVICE_LIB) $(DZ_DEVICE_LIB) $(ZC_DEVICE_LIB) $(LZ4F_DEVICE_LIB) $(LINK_LIBS) $(HLIF_SHIM_LIB) $(EMU_LIB)
 
 $(EMU_LIB): $(EMU_SRCS) $(wildcard tests/emu/*.h) $(wildcard tests/emu/*.cuh) $(wildcard tests/emu/nvcomp/device/detail/*.cuh) $(HDRS)
 	g++ -std=c++17 -O2 -g -fPIC -shared -Wall -Wno-unknown-pragmas -Wno-unused-function \
@@ -88,6 +91,19 @@ $(ZC_DEVICE_LIB): tests/cpp/zstd_compress_device_kernels.cu $(HDRS)
 	@mkdir -p build/tests
 	$(NVCC) $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -shared -Xptxas -v $< -o $@ \
 	    2> build/tests/libzstd_compress_device.ptxas.log || (cat build/tests/libzstd_compress_device.ptxas.log; exit 1)
+
+build/tests/liblz4frame_device.so: tests/cpp/lz4frame_device_kernels.cu $(HDRS)
+	@mkdir -p build/tests
+	$(NVCC) $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -shared -Xptxas -v $< -o $@ \
+	    2> build/tests/liblz4frame_device.ptxas.log || (cat build/tests/liblz4frame_device.ptxas.log; exit 1)
+
+# the same kernels built with -rdc=true and linked with a second translation unit over the same headers
+build/tests/lz4frame_rdc_%.o: tests/cpp/lz4frame_device_kernels.cu $(HDRS)
+	@mkdir -p build/tests
+	$(NVCC) $(ARCH) -O3 -std=c++17 -Xcompiler -fPIC,-Wall -Iinclude -rdc=true $(if $(filter 2,$*),-DLZ4F_LINK_ONLY) -c $< -o $@
+
+build/tests/liblz4frame_device_rdc.so: build/tests/lz4frame_rdc_1.o build/tests/lz4frame_rdc_2.o
+	$(NVCC) $(ARCH) -rdc=true -shared $^ -o $@
 
 build/tests/link_tu%.o: tests/cpp/device_headers_link.cu $(HDRS)
 	@mkdir -p build/tests

@@ -33,11 +33,15 @@ __device__ __forceinline__ bool lz4_read_ext(const uint8_t* __restrict__ in, uin
 
 // Walk the sequences of one LZ4 block without copying (size query: LZ4 blocks carry no size header).
 // Returns true on a well-formed block; *produced receives the decompressed size.
+// kHist (LZ4 frames, lz4frame_decode.cuh): the block starts at output position op0 of its frame, and a match may reach
+// back into those op0 earlier bytes; *produced is then the end position (op0 + the block's size).  Without kHist op0
+// is ignored and the block starts at 0.
+template <bool kHist = false>
 __device__ __forceinline__ bool lz4_walk_chunk(const uint8_t* __restrict__ in, uint32_t in_n,
-                                               uint32_t* produced, int lane) {
+                                               uint32_t* produced, int lane, uint32_t op0 = 0) {
   uint32_t ip = 0;
-  uint64_t op = 0;
-  if (in_n == 0) { *produced = 0; return true; }
+  uint64_t op = kHist ? op0 : 0;
+  if (in_n == 0) { *produced = (uint32_t)op; return true; }
   while (true) {
     if (ip >= in_n) return false;
     const uint32_t tok = in[ip++];
@@ -69,14 +73,18 @@ __device__ __forceinline__ bool lz4_walk_chunk(const uint8_t* __restrict__ in, u
 // no load from the output buffer.  Other matches are copied through memory (lz_common.cuh) with the fields
 // already in registers; sequences that do not fit the window (long literal runs, far length
 // extensions, the end of the block) take the generic field-by-field path below.
+// kHist (LZ4 frames): `out` is the frame's first output byte, the block starts at position op0 with the op0 bytes
+// before it final in global memory, matches may reach back into them, and out_cap64 and *produced are positions in
+// the frame (end of the block's room, end of the block).  Without kHist op0 is ignored and the block starts at 0.
 // ---------------------------------------------------------------------------
+template <bool kHist = false>
 __device__ __forceinline__ bool lz4_decode_chunk_direct(const uint8_t* __restrict__ in, uint32_t in_n,
                                                         uint8_t* out, uint64_t out_cap64,
-                                                        uint32_t* produced, int lane) {
-  if (in_n == 0) { *produced = 0; return true; }
+                                                        uint32_t* produced, int lane, uint32_t op0 = 0) {
+  if (in_n == 0) { *produced = kHist ? op0 : 0; return true; }
   const uint32_t cap = out_cap64 > 0xffffffffull ? 0xffffffffu : (uint32_t)out_cap64;
   const uint32_t ul = (uint32_t)lane;
-  uint32_t ip = 0, op = 0;
+  uint32_t ip = 0, op = kHist ? op0 : 0;
   while (true) {
     if (ip >= in_n) return false;
     if (ip + 32u <= in_n) {
@@ -200,6 +208,28 @@ __device__ __forceinline__ bool lz4_decode_chunk_v2(const uint8_t* in, uint32_t 
   s.cur = 0; s.pf_ip = kNoPrefetch; s.parity = tma_parity; s.next = kNextUnknown;
   const bool ok = lz_decode_stream<Lz4Decode>(s, lane);
   tma_parity = s.parity;                 // the barrier outlives the chunk: carry its phase to the next one
+  if (!ok) return false;
+  *produced = s.op;
+  return true;
+}
+
+// One block of a linked LZ4 frame (lz4frame_decode.cuh) with the block-parallel decoder: `out` is the frame's first
+// output byte, the block starts at position op0 with the op0 bytes before it final in global memory, and out_cap is
+// the end of the block's room as a position in the frame.  The decoder's state already keeps positions relative to
+// `out` and reads sources below ring_lo from global memory, so the history is only a starting state: op, flushed and
+// ring_lo at op0.  Matches may reach back to the frame's first byte.  *produced is the end position.
+__device__ __forceinline__ bool lz4_decode_block_v2_linked(const uint8_t* in, uint32_t in_n, uint8_t* out,
+                                                           uint64_t out_cap, uint32_t op0, uint32_t* produced,
+                                                           uint8_t* ring, uint32_t& tma_parity, int lane) {
+  if (in_n == 0) { *produced = op0; return true; }
+  LzState s;
+  s.in = in; s.in_n = in_n; s.out = out; s.out_cap = out_cap > 0xffffffffull ? 0xffffffffull : out_cap;
+  s.ip = 0; s.op = op0; s.flushed = op0; s.ring_lo = op0;
+  s.align = (uint32_t)((uintptr_t)out & 15u);
+  s.ring = smem_addr(ring);
+  s.cur = 0; s.pf_ip = kNoPrefetch; s.parity = tma_parity; s.next = kNextUnknown;
+  const bool ok = lz_decode_stream<Lz4Decode>(s, lane);
+  tma_parity = s.parity;
   if (!ok) return false;
   *produced = s.op;
   return true;

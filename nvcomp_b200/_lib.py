@@ -11,8 +11,8 @@ _LIB = None
 FORMATS = ("LZ4", "Snappy", "Cascaded", "Bitcomp", "ANS", "Deflate")
 
 # formats this library decodes but does not encode (streams from zlib, gzip, libzstd, Parquet / ORC writers, ...):
-# the three decompression entry points below are the ones they implement (include/nvcomp/gzip.h, zstd.h)
-DECODE_ONLY_FORMATS = ("Gzip", "Zstd")
+# the three decompression entry points below are the ones they implement (include/nvcomp/gzip.h, zstd.h, lz4frame.h)
+DECODE_ONLY_FORMATS = ("Gzip", "Zstd", "LZ4Frame")
 DECODE_ENTRY_POINTS = ("DecompressGetTempSize", "GetDecompressSizeAsync", "DecompressAsync")
 
 # the six (+2 Ex) entry points every format exports -- SURVEY.md section 8b

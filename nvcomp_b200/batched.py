@@ -104,8 +104,9 @@ def empty_batch(n: int, stride: int, device: str | torch.device = "cuda", align:
 
 
 class Codec:
-    """One format's six LLIF entry points, bound to raw pointers.  Gzip and Zstd (``_lib.DECODE_ONLY_FORMATS``) have
-    only the decompression half: their compress methods raise NotImplementedError."""
+    """One format's six LLIF entry points, bound to raw pointers.  Gzip, Zstd and LZ4Frame
+    (``_lib.DECODE_ONLY_FORMATS``) have only the decompression half: their compress methods raise
+    NotImplementedError."""
 
     def __init__(self, fmt: str, opts=None):
         self.decode_only = fmt in _lib.DECODE_ONLY_FORMATS
